@@ -625,8 +625,6 @@ __device__ __forceinline__ bool direct_leg_lost(const SimDev &d, uint32_t round,
   return bounded(word_of(y, (j - 1) & 3), 1000000u) < d.loss_ppm;
 }
 
-__device__ __forceinline__ void peer_publish_cta(const SimDev &d, uint32_t mail_round); // defined with the cross-GPU sync
-
 constexpr int kScanGroups = 2; // Philox groups (of 4 nodes) per lane per iteration: 8 nodes, 8 loads in flight
 
 __device__ __forceinline__ uint32_t ci(uint32_t round) { return round % 3u; } // slot of the per-round list counters
@@ -672,8 +670,6 @@ __device__ __forceinline__ uint32_t pick_target_warp(const SimDev &d, uint32_t (
   return pick_remove_warp<W>(am, bounded(word, L), lane);
 }
 
-// One node's tick decision from its meta words (what K1a does per node): counts the Ping and tells
-// whether the node needs K1b. Shared by the scan and by K1b's re-scan of last round's receivers.
 // The period's direct probes of one node (kRandomMembers store P [] — ONE shuffle, take P, Core.hs:239 — each target
 // pinged once): true if some target's Ack will not come back (the target process is down, or the leg is lost), i.e. the
 // node must go through K1b. `am` is consumed; L = popc(am) > 0.
@@ -698,24 +694,97 @@ __device__ __forceinline__ bool probe_fails(const SimDev &d, uint32_t (&am)[W], 
   return fails;
 }
 
-// One node's tick decision from its meta words (what K1a does per node): counts the Pings and tells
-// whether the node needs K1b. Shared by the scan (wide rows), the batched quiet scan and the receive pass.
+// A node's tick decision — does it need K1b in this round? A crashed process does nothing. A buffered record to send or
+// a countdown to run [Q8] means work. Otherwise only a failed probe can, and only if a crashed process sits in an Alive
+// slot or messages can be lost: then the probe decides (probe_fails, on the node's draws). Without either, whichever slot
+// a draw selects, the Ack comes back, so the picks and the Philox blocks behind them are not needed — the common case.
+// The rule is stated from a node's meta words by node_needs_work (the wide-row scan, the batched quiet scan and, with the
+// draws made early, the receive pass) and from a view row a warp has loaded by tick_decide and x_node; the W == 1 scan
+// restates it inline. Each form is written for the register budget of the kernels it sits in.
+
+// From the meta words; counts the node's Pings as well.
 template <int W>
 __device__ __forceinline__ bool node_needs_work(const SimDev &d, uint32_t flags, uint32_t (&am)[W], const uint32_t (&td)[W],
                                                 uint32_t sus, uint32_t tdraw, uint32_t ldraw, uint32_t round, uint32_t &pings,
                                                 uint32_t self) {
-  if ((flags & 0xFFu) == 0) return false;              // a crashed process does nothing
-  bool need = (flags & 0xFF00u) != 0 || sus != 0;       // piggyback to send, or a countdown to run [Q8]
+  if ((flags & 0xFFu) == 0) return false;
+  bool need = (flags & 0xFF00u) != 0 || sus != 0;
   uint32_t L = 0, risk = d.loss_ppm;
 #pragma unroll
   for (int w = 0; w < W; ++w) { L += __popc(am[w]); risk |= am[w] & td[w]; }
   if (L) {
     pings += d.P < L ? d.P : L;                                      // Ping (Core.hs:246), one per probe of the period
-    // No crashed process among the Alive slots and no message loss: whichever slot a draw selects, the Ack comes
-    // back, so the picks (and, in the scan, the Philox block behind `tdraw`) are not needed — the common case.
     if (risk) need |= probe_fails<W>(d, am, td, L, tdraw, ldraw, round, self);
   }
   return need;
+}
+
+// The tick decision of `tick_round` for a live local node from its freshly updated row (what K1a computes from the meta
+// record): counts its Pings and, if it needs K1b, appends it to that round's work list and marks it in `listbits`.
+template <int W>
+__device__ __forceinline__ void tick_decide(const SimDev &d, uint32_t tick_round, uint32_t ln, const Row<W> &row, uint32_t pbcnt,
+                                            const uint32_t (&td)[W], int lane, Ctr &c, uint32_t *listbits) {
+  const uint32_t self = d.first + ln;
+  uint32_t am[W], sus = 0, L = 0, risk = d.loss_ppm;
+#pragma unroll
+  for (int w = 0; w < W; ++w) {
+    am[w] = __ballot_sync(kFull, (row.st[w] & 3u) == SWIM_ALIVE);
+    sus |= __ballot_sync(kFull, (row.st[w] & 3u) == SWIM_SUSPECT);
+    L += __popc(am[w]);
+    risk |= am[w] & td[w];
+  }
+  bool need = pbcnt != 0 || sus != 0;
+  if (L && risk && !need) { // only now does the decision depend on the node's draws
+    const uint4 x = target_block<W>(d, tick_round, self >> 2);
+    uint32_t ldraw = 0;
+    if (d.loss_ppm) ldraw = word_of(philox4x32_10(make_uint4(tick_round, self >> 2, P_LOSS0, 0), d.key0, d.key1), self & 3);
+    need = probe_fails<W>(d, am, td, L, word_of(x, self & 3), ldraw, tick_round, self);
+  }
+  if (lane == 0) {
+    if (L) c.v[SWIM_CTR_PINGS] += d.P < L ? d.P : L;
+    if (need) {
+      wl_of(d, tick_round)[atomicAdd(&d.wl_cnt[ci(tick_round)], 1u)] = ln;
+      if (listbits) atomicOr(&listbits[ln >> 5], 1u << (ln & 31));
+    }
+  }
+}
+
+// The meta records (word 0) of the 4 U nodes a lane takes in one trip of a scan: m[u][j] = node 4 (gb + 32 u + lane) + j.
+// Returns the nodes that lie in the shard (bit 4 u + j).
+template <int W>
+__device__ __forceinline__ uint32_t load_meta_group(const SimDev &d, uint32_t gb, int lane, uint4 (&m)[kScanGroups][4]) {
+  constexpr int U = kScanGroups;
+  uint32_t valid = 0;
+  if (4 * gb >= d.first && 4 * (gb + 32 * U) <= d.first + d.n) { // an interior warp: all 128 U nodes are the shard's
+    const uint4 *p = d.meta + (size_t)(4 * (gb + lane) - d.first) * W;
+#pragma unroll
+    for (int u = 0; u < U; ++u)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) m[u][j] = p[(size_t)(u * 128 + j) * W]; // 4*U independent 16-byte loads in flight
+    valid = (1u << (4 * U)) - 1u;
+  } else {
+#pragma unroll
+    for (int u = 0; u < U; ++u)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint32_t node = 4 * (gb + u * 32 + lane) + j;
+        const bool ok = node >= d.first && node < d.first + d.n;
+        valid |= (uint32_t)ok << (u * 4 + j);
+        m[u][j] = ok ? d.meta[(size_t)(node - d.first) * W] : make_uint4(0, 0, 0, 0);
+      }
+  }
+  return valid;
+}
+
+// Local node l's bitmaps from its meta words: word 0 (m0) is already loaded, words 1 .. W-1 are loaded here.
+template <int W>
+__device__ __forceinline__ void node_meta(const SimDev &d, uint32_t l, uint4 m0, uint32_t (&am)[W], uint32_t (&td)[W], uint32_t &sus) {
+  am[0] = m0.x; td[0] = m0.z; sus = m0.y;
+#pragma unroll
+  for (int w = 1; w < W; ++w) {
+    const uint4 mw = d.meta[(size_t)l * W + w];
+    am[w] = mw.x; sus |= mw.y; td[w] = mw.z;
+  }
 }
 
 // K1a — streaming pass over every node of the shard, EIGHT nodes per lane: the four nodes 4g..4g+3
@@ -737,25 +806,7 @@ __device__ __forceinline__ void scan_pass(const SimDev &d, uint32_t round, uint3
   const uint32_t g0 = d.first >> 2, g1 = (d.first + d.n + 3) >> 2; // Philox groups touching this shard
   for (uint32_t gb = g0 + warp * (32 * U); gb < g1; gb += nwarps * (32 * U)) {
     uint4 m[U][4];
-    uint32_t valid = 0; // bit u*4+j
-    if (4 * gb >= d.first && 4 * (gb + 32 * U) <= d.first + d.n) { // an interior warp: all 128 U nodes are the shard's
-      const uint4 *p = d.meta + (size_t)(4 * (gb + lane) - d.first) * W;
-#pragma unroll
-      for (int u = 0; u < U; ++u)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) m[u][j] = p[(size_t)(u * 128 + j) * W]; // 4*U independent 16-byte loads in flight
-      valid = (1u << (4 * U)) - 1u;
-    } else {
-#pragma unroll
-      for (int u = 0; u < U; ++u)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const uint32_t node = 4 * (gb + u * 32 + lane) + j;
-          const bool ok = node >= d.first && node < d.first + d.n;
-          valid |= (uint32_t)ok << (u * 4 + j);
-          m[u][j] = ok ? d.meta[(size_t)(node - d.first) * W] : make_uint4(0, 0, 0, 0);
-        }
-    }
+    uint32_t valid = load_meta_group<W>(d, gb, lane, m); // bit u*4+j
     if ((skipbits || skipbits2) && valid == (1u << (4 * U)) - 1u && (d.first & 3u) == 0) {
       // (the lane's four nodes of a group are consecutive and 4-aligned in the shard: one bitmap word holds their bits)
 #pragma unroll
@@ -861,14 +912,8 @@ __device__ __forceinline__ void scan_pass(const SimDev &d, uint32_t round, uint3
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         if (!(valid >> (u * 4 + j) & 1u)) continue;
-        uint32_t am[W], td[W], sus = m[u][j].y;
-        am[0] = m[u][j].x; td[0] = m[u][j].z;
-        const uint32_t l = 4 * g + j - d.first;
-#pragma unroll
-        for (int w = 1; w < W; ++w) {
-          const uint4 mw = d.meta[(size_t)l * W + w];
-          am[w] = mw.x; sus |= mw.y; td[w] = mw.z;
-        }
+        uint32_t am[W], td[W], sus;
+        node_meta<W>(d, 4 * g + j - d.first, m[u][j], am, td, sus);
         const bool need = node_needs_work<W>(d, m[u][j].w, am, td, sus, word_of(x, j), word_of(y, j), round, pings, 4 * g + j);
         work |= (uint32_t)need << (u * 4 + j);
       }
@@ -932,41 +977,15 @@ __device__ __forceinline__ uint32_t quiet_scan(const SimDev &d, uint32_t round, 
   const uint32_t g0 = d.first >> 2, g1 = (d.first + d.n + 3) >> 2;
   for (uint32_t gb = g0 + warp * (32 * U); gb < g1; gb += nwarps * (32 * U)) {
     uint4 m[U][4];
-    uint32_t valid = 0;
-    if (4 * gb >= d.first && 4 * (gb + 32 * U) <= d.first + d.n) { // an interior warp (see scan_pass)
-      const uint4 *p = d.meta + (size_t)(4 * (gb + lane) - d.first) * W;
-#pragma unroll
-      for (int u = 0; u < U; ++u)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) m[u][j] = p[(size_t)(u * 128 + j) * W];
-      valid = (1u << (4 * U)) - 1u;
-    } else {
-#pragma unroll
-      for (int u = 0; u < U; ++u)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const uint32_t node = 4 * (gb + u * 32 + lane) + j;
-          const bool ok = node >= d.first && node < d.first + d.n;
-          valid |= (uint32_t)ok << (u * 4 + j);
-          m[u][j] = ok ? d.meta[(size_t)(node - d.first) * W] : make_uint4(0, 0, 0, 0);
-        }
-    }
+    const uint32_t valid = load_meta_group<W>(d, gb, lane, m);
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       const uint32_t g = gb + u * 32 + lane;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         if (!(valid >> (u * 4 + j) & 1u)) continue;
-        uint32_t am[W], td[W], sus = m[u][j].y, risk = 0;
-        am[0] = m[u][j].x; td[0] = m[u][j].z;
-        if (W > 1) {
-          const uint32_t l = 4 * g + j - d.first;
-#pragma unroll
-          for (int w = 1; w < W; ++w) {
-            const uint4 mw = d.meta[(size_t)l * W + w];
-            am[w] = mw.x; sus |= mw.y; td[w] = mw.z;
-          }
-        }
+        uint32_t am[W], td[W], sus, risk = 0;
+        node_meta<W>(d, 4 * g + j - d.first, m[u][j], am, td, sus);
 #pragma unroll
         for (int w = 0; w < W; ++w) risk |= am[w] & td[w];
         if (!risk) { // the draw is never looked at: one decision for the whole batch
@@ -1294,50 +1313,31 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) tick_work_kernel(SimDev 
 }
 
 // =================================================================== cross-GPU synchronisation
-// Fused exchange: before a rank applies round `mail_round`'s mail it must know that every peer has
-// finished K1b of that round (all flags / stamps / list entries have landed in its memory) and how
-// many receivers each peer listed. CTA 0 publishes (after griddepcontrol.wait, i.e. after this rank's
-// own K1b completed): per-peer counts, then the round number into word [rank] of every peer's barrier
-// array. Every warp that is about to receive waits until all words of its own array reached the round.
-// The wait is bounded: a missing peer sets *bar_err instead of hanging the GPU.
-__device__ __forceinline__ void peer_publish(const SimDev &d, uint32_t mail_round) {
-  if (blockIdx.x != 0) return;
-  peer_publish_cta(d, mail_round);
-}
-
-// threads q < world of the calling CTA publish to peer q
-__device__ __forceinline__ void peer_publish_cta(const SimDev &d, uint32_t mail_round) {
+// Fused exchange: before a rank applies round `mail_round`'s mail it must know that every peer has finished K1b of that
+// round (all flags / list entries have landed in its memory) and how many receivers each peer listed there.
+// peer_handshake_cta is run by ALL threads of one CTA, once every CTA of this rank has finished its K1b of the round and
+// those that stored into peer memory have fenced at system scope: the last CTA to arrive at a grid barrier of the round
+// kernels, or peer_barrier_kernel. Thread q publishes to peer q the number of receivers this rank listed there and then,
+// with release semantics, this rank's round word; it then waits (acquire) for peer q's word. One thread per peer, all
+// peers in parallel; the wait is bounded (a missing peer sets *bar_err instead of hanging the GPU).
+__device__ __forceinline__ void peer_handshake_cta(const SimDev &d, uint32_t mail_round) {
   const uint32_t q = threadIdx.x;
-  if (q >= d.world) return;
-  if (q != d.rank) {
-    d.rcnt_p[q][(mail_round & 1) * d.world + d.rank] = d.xcnt[q];
-    d.xcnt[q] = 0;
-  }
-  // release: this rank's mail of the round (K1b completed before this kernel started) and the count above are visible to
-  // whoever acquires the round word
-  st_release_sys(d.bar_p[q] + d.rank, mail_round);
-}
-
-__device__ __forceinline__ void peer_wait(const SimDev &d, uint32_t mail_round, int lane) {
-  if ((uint32_t)lane < d.world) {
-    const uint32_t *mine = d.bar_p[d.rank] + lane;
+  if (q < d.world && q != d.rank) {
+    d.rcnt_p[q][(mail_round & 1) * d.world + d.rank] = atomicExch(&d.xcnt[q], 0u);
+    st_release_sys(d.bar_p[q] + d.rank, mail_round);
+    const uint32_t *mine = d.bar_p[d.rank] + q;
     const long long t0 = clock64();
     uint32_t polls = 0;
-    while ((int32_t)(ld_acquire_sys(mine) - mail_round) < 0) {
+    while ((int32_t)(ld_acquire_sys(mine) - mail_round) < 0)
       if (wait_expired(d, t0, kPeerWaitCycles, polls, 1)) break; // a peer stopped stepping
-      __nanosleep(100);
-    }
   }
-  __syncwarp();
 }
 
-// stand-alone form of the same synchronisation (default path): one warp, launched between K1b and K2
+// stand-alone form of the same synchronisation (split launch sequence): one CTA, launched between K1b and K2
 static __global__ void peer_barrier_kernel(SimDev d) {
   pdl_launch();
   pdl_wait(); // K1b of this rank is complete and flushed
-  const uint32_t round = d.round;
-  peer_publish(d, round);
-  peer_wait(d, round, (int)threadIdx.x);
+  peer_handshake_cta(d, d.round);
 }
 
 // =================================================================== K2: receive
@@ -1455,15 +1455,15 @@ __device__ __forceinline__ void recv_one(const SimDev &d, uint32_t round, uint32
   }
 }
 
-// warp-per-receiver over the receivers of `round`: the compact list of delivered slots K1b wrote, then one list per
-// source rank (cross-shard senders). A receiver can be listed more
-// than once: the claim stamp lets exactly one warp process it.
-template <int W>
-__device__ __forceinline__ void recv_pass(const SimDev &d, uint32_t round, uint32_t warp, uint32_t nwarps,
-                                          int lane, PbStage &pbs, Ctr &c, uint32_t tick_round = 0) {
+// Warp-per-receiver walk over the receivers of `round`, f(ln, early, snd) for each: the compact list of delivered slots
+// K1b wrote (early = true: the slot names one sender, snd, whose snapshot can be fetched with the row), then one list per
+// source rank (cross-shard senders). A receiver can be listed more than once: the claim stamp lets exactly one warp
+// process it.
+template <typename F>
+__device__ __forceinline__ void for_each_receiver(const SimDev &d, uint32_t round, uint32_t warp, uint32_t nwarps, F f) {
   const uint32_t par = round & 1;
-  // items go to the warps from the top down: in the fused kernel this pass shares a phase with the scan, whose node ranges
-  // fill the warps from the bottom up (at C3 the last 640 of 4736 warps have no nodes to scan)
+  // items go to the warps from the top down: in the fused kernels the walk shares a phase with the scan, whose node ranges
+  // fill the warps from the bottom up (at C3 the last 128 of 4,224 warps have no nodes to scan)
   const uint32_t w0 = nwarps - 1 - warp;
   const uint2 *cl_in = d.cl + (size_t)par * d.n * d.fanout;
   // this warp's first entry travels with the list's length (one memory round trip instead of two); only looked at if w0 < n_cl
@@ -1475,7 +1475,7 @@ __device__ __forceinline__ void recv_pass(const SimDev &d, uint32_t round, uint3
   const uint32_t n_cl = d.ncand[ci(round)];
   for (uint32_t item = w0; item < n_cl; item += nwarps) {
     const uint2 e = item == w0 ? e_first : cl_in[item];
-    recv_one<W>(d, round, e.x, true, e.y, lane, pbs, c, tick_round);
+    f(e.x, true, e.y);
   }
   if (d.world > 1) {
     uint32_t seg_end[SWIM_MAX_WORLD + 1];
@@ -1488,10 +1488,17 @@ __device__ __forceinline__ void recv_pass(const SimDev &d, uint32_t round, uint3
     for (uint32_t item = w0; item < n_recv; item += nwarps) {
       uint32_t a = 0;
       while (item >= seg_end[1 + a]) ++a;
-      const uint32_t ln = d.rlr[((size_t)par * d.world + a) * d.rcap + (item - seg_end[a])];
-      recv_one<W>(d, round, ln, false, 0u, lane, pbs, c, tick_round);
+      f(d.rlr[((size_t)par * d.world + a) * d.rcap + (item - seg_end[a])], false, 0u);
     }
   }
+}
+
+template <int W>
+__device__ __forceinline__ void recv_pass(const SimDev &d, uint32_t round, uint32_t warp, uint32_t nwarps,
+                                          int lane, PbStage &pbs, Ctr &c, uint32_t tick_round = 0) {
+  for_each_receiver(d, round, warp, nwarps, [&](uint32_t ln, bool early, uint32_t snd) {
+    recv_one<W>(d, round, ln, early, snd, lane, pbs, c, tick_round);
+  });
 }
 
 // stand-alone K2 (profiling, staged NCCL exchange, sharded runs)
@@ -1523,46 +1530,76 @@ __device__ __forceinline__ uint32_t *barrier_generation() {
 __device__ __forceinline__ void barrier_begin(const SimDev &d) {
   if (threadIdx.x == 0) *barrier_generation() = *(volatile uint32_t *)(d.gbar + 1);
 }
-__device__ __forceinline__ void grid_barrier(const SimDev &d, uint32_t tl_round = 0, int tl_slot = -1) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    volatile uint32_t *gen = d.gbar + 1;
-    const uint32_t g = (*barrier_generation())++;
-    __threadfence();
-    if (atomicAdd(d.gbar, 1u) == gridDim.x - 1) {
-      tl_mark_last(d, tl_round, tl_slot);
-      d.gbar[0] = 0;
-      __threadfence();
-      atomicAdd(d.gbar + 1, 1u);
-    } else {
-      const long long t0 = clock64();
-      uint32_t polls = 0;
-      while (*gen == g) {
-        if (wait_expired(d, t0, 6000000000ll, polls, 2)) break;
-        __nanosleep(20);
-      }
-    }
-    __threadfence();
-  }
-  __syncthreads();
+// The grid barrier. Thread 0 of every CTA arrives behind a fence (at system scope with fence_sys: this CTA stored into
+// peer memory since the last barrier); the last CTA to arrive does the barrier's job, if it has one, and releases the
+// grid, while the others spin on the generation word. The jobs:
+//   * cnt_dst: freeze a work-list length, *cnt_src -> *cnt_dst (round_kernel_x);
+//   * kHandshake: the cross-GPU handshake of `round` (peer_handshake_cta, by all threads of the last CTA), if want() —
+//     evaluated by the last CTA only, after every arrival is visible — says it is due (round_kernel folds it into the scan
+//     barrier of a round that listed no work).
+// Without kHandshake the barrier stays with thread 0 of each CTA: the form for call sites that cannot shard. The wait
+// gives up after 6e9 cycles, or kPeerWaitCycles more where the last CTA may be handshaking. tl_slot: timeline slot of the
+// last arrival (tl_mark_last).
+struct Always {
+  __device__ bool operator()() const { return true; }
+};
+// the last arrival's release of the grid, and everybody else's bounded wait for it (thread 0 of a CTA)
+__device__ __forceinline__ void barrier_release(const SimDev &d, const uint32_t *cnt_src, uint32_t *cnt_dst) {
+  if (cnt_dst) *(volatile uint32_t *)cnt_dst = *(volatile const uint32_t *)cnt_src;
+  d.gbar[0] = 0;
+  __threadfence();
+  atomicAdd(d.gbar + 1, 1u);
 }
-
-// The cross-GPU handshake of round `mail_round`, run by ALL threads of one CTA (the last one to arrive at a grid barrier —
-// by then every CTA of this rank has finished its K1b of the round, and those that stored into peer memory have fenced
-// at system scope): thread q publishes to peer q the number of receivers this rank listed there and then, with release
-// semantics, this rank's round word; it then waits (acquire) for peer q's word. One thread per peer, all peers in
-// parallel; the wait is bounded (a missing peer sets *bar_err instead of hanging the GPU).
-__device__ __forceinline__ void peer_handshake_cta(const SimDev &d, uint32_t mail_round) {
-  const uint32_t q = threadIdx.x;
-  if (q < d.world && q != d.rank) {
-    d.rcnt_p[q][(mail_round & 1) * d.world + d.rank] = atomicExch(&d.xcnt[q], 0u);
-    st_release_sys(d.bar_p[q] + d.rank, mail_round);
-    const uint32_t *mine = d.bar_p[d.rank] + q;
-    const long long t0 = clock64();
-    uint32_t polls = 0;
-    while ((int32_t)(ld_acquire_sys(mine) - mail_round) < 0)
-      if (wait_expired(d, t0, kPeerWaitCycles, polls, 1)) break; // a peer stopped stepping
+__device__ __forceinline__ void barrier_wait(const SimDev &d, volatile uint32_t *gen, uint32_t g, long long limit) {
+  const long long t0 = clock64();
+  uint32_t polls = 0;
+  while (*gen == g) {
+    if (wait_expired(d, t0, limit, polls, 2)) break;
+    __nanosleep(20);
   }
+}
+template <bool kHandshake = false, typename Want = Always>
+__device__ __forceinline__ void grid_barrier(const SimDev &d, uint32_t round = 0, int tl_slot = -1, const uint32_t *cnt_src = nullptr,
+                                             uint32_t *cnt_dst = nullptr, bool fence_sys = false, Want want = Want()) {
+  __syncthreads();
+  if constexpr (!kHandshake) {
+    if (threadIdx.x == 0) {
+      volatile uint32_t *gen = d.gbar + 1;
+      const uint32_t g = (*barrier_generation())++;
+      __threadfence();
+      if (atomicAdd(d.gbar, 1u) == gridDim.x - 1) {
+        if (cnt_dst) __threadfence(); // acquire side of the arrivals, ahead of the job
+        tl_mark_last(d, round, tl_slot);
+        barrier_release(d, cnt_src, cnt_dst);
+      } else {
+        barrier_wait(d, gen, g, 6000000000ll);
+      }
+      __threadfence();
+    }
+  } else {
+    SWIM_SHARED_1D(uint32_t, s_last, 1);
+    if (threadIdx.x == 0) {
+      if (fence_sys) __threadfence_system(); else __threadfence();
+      const bool last = atomicAdd(d.gbar, 1u) == gridDim.x - 1;
+      if (last) { __threadfence(); tl_mark_last(d, round, tl_slot); } // acquire side of the arrivals
+      s_last[0] = last ? 1u : 0u;
+    }
+    __syncthreads();
+    if (s_last[0]) {
+      if (want()) peer_handshake_cta(d, round);
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        (*barrier_generation())++;
+        barrier_release(d, cnt_src, cnt_dst);
+      }
+    } else if (threadIdx.x == 0) {
+      volatile uint32_t *gen = d.gbar + 1;
+      const uint32_t g = (*barrier_generation())++;
+      barrier_wait(d, gen, g, kPeerWaitCycles + 6000000000ll);
+      __threadfence();
+    }
+  }
+  __syncthreads();
 }
 
 // CTA-wide OR of a per-thread predicate (every thread of the CTA must call it)
@@ -1575,43 +1612,9 @@ __device__ __forceinline__ bool cta_or(bool pred) {
   return s_or[0] != 0;
 }
 
-// grid_barrier with a job for the last CTA to arrive: `handshake` = 0 none, else the round whose cross-GPU handshake that
-// CTA performs before it releases the grid (everybody else spins on the local generation word as in grid_barrier).
-// fence_sys: this CTA stored into peer memory since the last barrier (its arrival must order those stores system-wide).
-// want(): evaluated by the last CTA only, after every arrival is visible — whether the handshake is due at this barrier
-// (round_kernel folds it into the scan barrier of a round that listed no work).
-template <typename Want>
-__device__ __forceinline__ void grid_barrier_leader(const SimDev &d, bool fence_sys, uint32_t mail_round, Want want, int tl_slot = -1) {
-  SWIM_SHARED_1D(uint32_t, s_last, 1);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    if (fence_sys) __threadfence_system(); else __threadfence();
-    const bool last = atomicAdd(d.gbar, 1u) == gridDim.x - 1;
-    if (last) { __threadfence(); tl_mark_last(d, mail_round, tl_slot); } // acquire side of the arrivals
-    s_last[0] = last ? 1u : 0u;
-  }
-  __syncthreads();
-  if (s_last[0]) {
-    if (want()) peer_handshake_cta(d, mail_round);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      (*barrier_generation())++;
-      d.gbar[0] = 0;
-      __threadfence();
-      atomicAdd(d.gbar + 1, 1u);
-    }
-  } else if (threadIdx.x == 0) {
-    volatile uint32_t *gen = d.gbar + 1;
-    const uint32_t g = (*barrier_generation())++;
-    const long long t0 = clock64();
-    uint32_t polls = 0;
-    while (*gen == g) {
-      if (wait_expired(d, t0, kPeerWaitCycles + 6000000000ll, polls, 2)) break;
-      __nanosleep(20);
-    }
-    __threadfence();
-  }
-  __syncthreads();
+// zero one slot (mbw words) of a per-node bitmap — mailbits, workbits —, grid-strided over the warps of the launch
+__device__ __forceinline__ void clear_bitmap(const SimDev &d, uint32_t *bits, uint32_t warp, uint32_t nwarps, int lane) {
+  for (uint32_t x = warp * 32 + lane; x < d.mbw; x += nwarps * 32) bits[x] = 0;
 }
 
 template <int W>
@@ -1679,22 +1682,20 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel(SimDev d) {
     const uint32_t *wl_cnt_r = d.wl_cnt + ci(round);
     // the work list is complete. Sharded: a rank that listed nothing has no K1b to run, so its cross-GPU handshake of the
     // round happens right here, inside this barrier (one barrier for a quiet round)
-    if (sharded) grid_barrier_leader(d, false, round, [&] { return *(volatile const uint32_t *)wl_cnt_r == 0; }, 5);
+    if (sharded) grid_barrier<true>(d, round, 5, nullptr, nullptr, false, [&] { return *(volatile const uint32_t *)wl_cnt_r == 0; });
     else grid_barrier(d, round, 5);
     tl_mark(d, round, 2);
     const uint32_t n_work = d.wl_cnt[ci(round)];
     const uint32_t first_ln = first_work_entry(d, round, warp);                  // in flight together with the count
-    if (mail) { // last round's mail bitmap has been read by every scanner: clear it (its next writers: senders of round + 2)
-      uint32_t *mb = d.mailbits + (size_t)((round - 1) % 3u) * d.mbw;
-      for (uint32_t x = warp * 32 + lane; x < d.mbw; x += nwarps * 32) mb[x] = 0;
-    }
+    // last round's mail bitmap has been read by every scanner: clear it (its next writers: senders of round + 2)
+    if (mail) clear_bitmap(d, d.mailbits + (size_t)((round - 1) % 3u) * d.mbw, warp, nwarps, lane);
     prev_quiet = n_work == 0 && !mail;
     // ---- phase W
     if (n_work) {
       const bool remote = work_pass<W>(d, round, warp, nwarps, lane, pbs, c, first_ln, false); // K1b
       tl_mark(d, round, 3);
       // every flag and snapshot is written; sharded: ... on every rank (the last CTA talks to the peers)
-      if (sharded) grid_barrier_leader(d, cta_or(remote), round, [] { return true; }, 6);
+      if (sharded) grid_barrier<true>(d, round, 6, nullptr, nullptr, cta_or(remote));
       else grid_barrier(d, round, 6);
       tl_mark(d, round, 4);
     }
@@ -1711,8 +1712,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel(SimDev d) {
   if (mail) { // the last round's mail, before the launch ends (no tick decision: the next launch scans everybody)
     recv_pass<W>(d, d.round + d.nrounds - 1, warp, nwarps, lane, pbs, c, 0);
     // its bitmap is not needed by anybody: clear it. (The receive pass does not read it, so no barrier in between.)
-    uint32_t *mb = d.mailbits + (size_t)((d.round + d.nrounds - 1) % 3u) * d.mbw;
-    for (uint32_t x = warp * 32 + lane; x < d.mbw; x += nwarps * 32) mb[x] = 0;
+    clear_bitmap(d, d.mailbits + (size_t)((d.round + d.nrounds - 1) % 3u) * d.mbw, warp, nwarps, lane);
   }
   c.flush(d.ctr, lane);
 }
@@ -1731,36 +1731,6 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel(SimDev d) {
 // warp per interval, mail flags and snapshots are round-parity double-buffered, and the bitmaps (mail of round r in slot
 // r % 3, work list of round r in slot r % 3) are cleared one interval after their last reader and one before their next
 // writer. Result: bit-identical to round_kernel, one barrier (and one cross-GPU handshake) per round instead of two.
-
-// The tick decision of `tick_round` for a live local node from its freshly updated row (what K1a computes from the meta
-// record): counts its Pings and, if it needs K1b, appends it to that round's work list and marks it in `listbits`.
-template <int W>
-__device__ __forceinline__ void tick_decide(const SimDev &d, uint32_t tick_round, uint32_t ln, const Row<W> &row, uint32_t pbcnt,
-                                            const uint32_t (&td)[W], int lane, Ctr &c, uint32_t *listbits) {
-  const uint32_t self = d.first + ln;
-  uint32_t am[W], sus = 0, L = 0, risk = d.loss_ppm;
-#pragma unroll
-  for (int w = 0; w < W; ++w) {
-    am[w] = __ballot_sync(kFull, (row.st[w] & 3u) == SWIM_ALIVE);
-    sus |= __ballot_sync(kFull, (row.st[w] & 3u) == SWIM_SUSPECT);
-    L += __popc(am[w]);
-    risk |= am[w] & td[w];
-  }
-  bool need = pbcnt != 0 || sus != 0;
-  if (L && risk && !need) { // only now does the decision depend on the node's draws
-    const uint4 x = target_block<W>(d, tick_round, self >> 2);
-    uint32_t ldraw = 0;
-    if (d.loss_ppm) ldraw = word_of(philox4x32_10(make_uint4(tick_round, self >> 2, P_LOSS0, 0), d.key0, d.key1), self & 3);
-    need = probe_fails<W>(d, am, td, L, word_of(x, self & 3), ldraw, tick_round, self);
-  }
-  if (lane == 0) {
-    if (L) c.v[SWIM_CTR_PINGS] += d.P < L ? d.P : L;
-    if (need) {
-      wl_of(d, tick_round)[atomicAdd(&d.wl_cnt[ci(tick_round)], 1u)] = ln;
-      if (listbits) atomicOr(&listbits[ln >> 5], 1u << (ln & 31));
-    }
-  }
-}
 
 // One node of the interval of round `round` (see above). from_wl: the node is item `idx` of the round's work list; else it
 // is a receiver of round - 1 named by a delivered slot (early / snd as in recv_one). mail: round - 1 delivered mail to
@@ -1849,69 +1819,6 @@ __device__ __forceinline__ void x_node(const SimDev &d, uint32_t round, uint32_t
   if (decide) tick_decide<W>(d, round + 1, ln, row, pbs.cnt, td, lane, c, d.workbits + (size_t)((round + 1) % 3u) * d.mbw);
 }
 
-// grid barrier whose last arrival also freezes a work-list length (*cnt_src -> *cnt_dst) before it releases the grid
-__device__ __forceinline__ void grid_barrier_freeze(const SimDev &d, const uint32_t *cnt_src, uint32_t *cnt_dst, uint32_t tl_round, int tl_slot) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    volatile uint32_t *gen = d.gbar + 1;
-    const uint32_t g = (*barrier_generation())++;
-    __threadfence();
-    if (atomicAdd(d.gbar, 1u) == gridDim.x - 1) {
-      __threadfence();
-      tl_mark_last(d, tl_round, tl_slot);
-      *(volatile uint32_t *)cnt_dst = *(volatile const uint32_t *)cnt_src;
-      d.gbar[0] = 0;
-      __threadfence();
-      atomicAdd(d.gbar + 1, 1u);
-    } else {
-      const long long t0 = clock64();
-      uint32_t polls = 0;
-      while (*gen == g) {
-        if (wait_expired(d, t0, 6000000000ll, polls, 2)) break;
-        __nanosleep(20);
-      }
-    }
-    __threadfence();
-  }
-  __syncthreads();
-}
-
-// the same with the cross-GPU handshake of `mail_round` performed by the last CTA to arrive (see grid_barrier_leader)
-__device__ __forceinline__ void grid_barrier_leader_freeze(const SimDev &d, bool fence_sys, uint32_t mail_round, const uint32_t *cnt_src,
-                                                           uint32_t *cnt_dst, int tl_slot) {
-  SWIM_SHARED_1D(uint32_t, s_last, 1);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    if (fence_sys) __threadfence_system(); else __threadfence();
-    const bool last = atomicAdd(d.gbar, 1u) == gridDim.x - 1;
-    if (last) { __threadfence(); tl_mark_last(d, mail_round, tl_slot); }
-    s_last[0] = last ? 1u : 0u;
-  }
-  __syncthreads();
-  if (s_last[0]) {
-    peer_handshake_cta(d, mail_round);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      (*barrier_generation())++;
-      *(volatile uint32_t *)cnt_dst = *(volatile const uint32_t *)cnt_src;
-      d.gbar[0] = 0;
-      __threadfence();
-      atomicAdd(d.gbar + 1, 1u);
-    }
-  } else if (threadIdx.x == 0) {
-    volatile uint32_t *gen = d.gbar + 1;
-    const uint32_t g = (*barrier_generation())++;
-    const long long t0 = clock64();
-    uint32_t polls = 0;
-    while (*gen == g) {
-      if (wait_expired(d, t0, kPeerWaitCycles + 6000000000ll, polls, 2)) break;
-      __nanosleep(20);
-    }
-    __threadfence();
-  }
-  __syncthreads();
-}
-
 template <int W>
 __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d) {
   SWIM_SHARED_2D(uint4, s_pb, kWarpsPerBlock, 32);
@@ -1941,21 +1848,17 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d)
       uint32_t pings = 0;
       scan_pass<W>(d, round, warp, nwarps, lane, pings, nullptr, pbs.s, nullptr, d.workbits + (size_t)(round % 3u) * d.mbw);
       c.v[SWIM_CTR_PINGS] += pings;
-      grid_barrier_freeze(d, d.wl_cnt + ci(round), d.wl_n + ci(round), round, -1);
+      grid_barrier(d, round, -1, d.wl_cnt + ci(round), d.wl_n + ci(round));
       have_wl = true;
       known_empty = false;
     }
     tl_mark(d, round, 0);
     const uint32_t n_work = known_empty ? 0u : *(volatile const uint32_t *)&d.wl_n[ci(round)];
     const bool last = round == last_round;
-    if (wb_prev) { // the bitmap of the work list of round - 1: read in the last interval, written again in the next one
-      uint32_t *wb = d.workbits + (size_t)((round - 1) % 3u) * d.mbw;
-      for (uint32_t x = warp * 32 + lane; x < d.mbw; x += nwarps * 32) wb[x] = 0;
-    }
-    if (mail_prev) { // the mail bitmap of round - 2 likewise (its next writers: the senders of round + 1)
-      uint32_t *mb = d.mailbits + (size_t)((round - 2) % 3u) * d.mbw;
-      for (uint32_t x = warp * 32 + lane; x < d.mbw; x += nwarps * 32) mb[x] = 0;
-    }
+    // the bitmap of the work list of round - 1: read in the last interval, written again in the next one; the mail bitmap
+    // of round - 2 likewise (its next writers: the senders of round + 1)
+    if (wb_prev) clear_bitmap(d, d.workbits + (size_t)((round - 1) % 3u) * d.mbw, warp, nwarps, lane);
+    if (mail_prev) clear_bitmap(d, d.mailbits + (size_t)((round - 2) % 3u) * d.mbw, warp, nwarps, lane);
     if (batching && n_work == 0 && !mail && !last) {
       // `round` is quiet — nothing to apply, nothing to run — and so committed. One pass decides rounds round+1 .. round+Q.
       // (No list is appended to and no mail counted while rounds are quiet: all counters of the three slots are cleared.)
@@ -2030,8 +1933,8 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d)
     }
     tl_mark(d, round, 1);
     // every flag, snapshot and list entry of the round is written (sharded: ... on every rank — the last CTA talks to the peers)
-    if (sharded) grid_barrier_leader_freeze(d, cta_or(did_remote), round, d.wl_cnt + ci(round + 1), d.wl_n + ci(round + 1), 5);
-    else grid_barrier_freeze(d, d.wl_cnt + ci(round + 1), d.wl_n + ci(round + 1), round, 5);
+    if (sharded) grid_barrier<true>(d, round, 5, d.wl_cnt + ci(round + 1), d.wl_n + ci(round + 1), cta_or(did_remote));
+    else grid_barrier(d, round, 5, d.wl_cnt + ci(round + 1), d.wl_n + ci(round + 1));
     tl_mark(d, round, 2);
     tl_mark(d, round, 4, (unsigned long long)(n_work || mail)); // 1: a busy round (bench.py tells busy from quiet rounds by it)
     mail_prev = mail;
@@ -2048,11 +1951,9 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d)
   if (mail) recv_pass<W>(d, last_round, warp, nwarps, lane, pbs, c, 0);
   // bitmaps still set: the mail of the last two rounds and the work lists (this rank's own affair: all three slots). Never
   // the mail slot of last + 1: a peer that is already in its next launch may be marking receivers there.
-  for (uint32_t x = warp * 32 + lane; x < d.mbw; x += nwarps * 32) {
-    d.mailbits[(size_t)(last_round % 3u) * d.mbw + x] = 0;
-    d.mailbits[(size_t)((last_round + 2u) % 3u) * d.mbw + x] = 0; // (= last - 1)
-    d.workbits[x] = 0; d.workbits[d.mbw + x] = 0; d.workbits[2 * (size_t)d.mbw + x] = 0;
-  }
+  clear_bitmap(d, d.mailbits + (size_t)(last_round % 3u) * d.mbw, warp, nwarps, lane);
+  clear_bitmap(d, d.mailbits + (size_t)((last_round + 2u) % 3u) * d.mbw, warp, nwarps, lane); // (= last - 1)
+  for (uint32_t s = 0; s < 3; ++s) clear_bitmap(d, d.workbits + (size_t)s * d.mbw, warp, nwarps, lane);
   c.flush(d.ctr, lane);
 }
 

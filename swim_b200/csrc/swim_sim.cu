@@ -621,7 +621,7 @@ static int run_rounds(swim_sim *sim, uint32_t rounds) {
   size_t ev_pos = 0;
   // Default: one kernel per round. The split sequence (K1a, K1b, [exchange], K2 as separate launches) serves
   // per-kernel profiling, the staged NCCL exchange and SWIM_SPLIT=1.
-  // Sharded runs with the fused exchange: round_kernel too (grid_barrier_leader: the last CTA to arrive at the barrier after
+  // Sharded runs with the fused exchange: round_kernel too (grid_barrier<true>: the last CTA to arrive at the barrier after
   // K1b — or at the scan barrier of a round without work — does the cross-GPU handshake, one thread per peer);
   // SWIM_ROUND_KERNEL=0 selects the split sequence + peer_barrier_kernel instead.
   const bool single_kernel = !sim->profile && !sim->opt_split &&
