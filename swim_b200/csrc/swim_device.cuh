@@ -581,9 +581,16 @@ __device__ __forceinline__ int row_apply(Row<W> &r, const SimDev &d, uint32_t se
 }
 
 // ------------------------------------------------------------------ counters
+// A thread's counters live in shared memory, not in registers: the round kernels keep them for the whole launch, and
+// eleven registers held across every pass pushed the passes' own values out to local memory. Thread t owns words
+// t * SWIM_CTR__COUNT ..; the stride is odd, so the 32 lanes of a warp hit 32 different banks.
+static_assert(SWIM_CTR__COUNT % 2 == 1, "per-thread counter slots must have an odd stride");
 struct Ctr {
-  uint32_t v[SWIM_CTR__COUNT];
+  uint32_t *v;
+  // binds this thread's slot and zeroes it; every kernel that uses Ctr runs CTAs of kThreads threads
   __device__ __forceinline__ void clear() {
+    SWIM_SHARED_1D(uint32_t, s_slots, kThreads * SWIM_CTR__COUNT);
+    v = s_slots + threadIdx.x * SWIM_CTR__COUNT;
 #pragma unroll
     for (int i = 0; i < SWIM_CTR__COUNT; ++i) v[i] = 0;
   }
@@ -807,6 +814,17 @@ __device__ __forceinline__ void scan_pass(const SimDev &d, uint32_t round, uint3
   for (uint32_t gb = g0 + warp * (32 * U); gb < g1; gb += nwarps * (32 * U)) {
     uint4 m[U][4];
     uint32_t valid = load_meta_group<W>(d, gb, lane, m); // bit u*4+j
+    uint32_t up = 0, busy = 0; // W == 1, bit u*4+j: the node's process is up / its record alone sends it to K1b
+    if constexpr (W == 1) {
+      // of a record, pass 1 below needs x, z and these two bits: folded right away, the eight records take 16 registers
+      // instead of 32 for the rest of the trip
+#pragma unroll
+      for (int q = 0; q < 4 * U; ++q) {
+        const uint4 mr = m[q >> 2][q & 3];
+        up |= (uint32_t)((mr.w & 0xFFu) != 0) << q;
+        busy |= (uint32_t)((mr.w & 0xFF00u) != 0 || mr.y != 0) << q;
+      }
+    }
     if ((skipbits || skipbits2) && valid == (1u << (4 * U)) - 1u && (d.first & 3u) == 0) {
       // (the lane's four nodes of a group are consecutive and 4-aligned in the shard: one bitmap word holds their bits)
 #pragma unroll
@@ -850,9 +868,9 @@ __device__ __forceinline__ void scan_pass(const SimDev &d, uint32_t round, uint3
           const int q = u * 4 + j;
           const uint4 mr = m[u][j];
           bool rq = false;
-          if ((valid >> q & 1u) && (mr.w & 0xFFu) != 0) { // in range, not left to the receive pass, process up
+          if (valid >> q & up >> q & 1u) { // in range, not left to the receive pass, process up
             const uint32_t L = __popc(mr.x);
-            const bool wk = (mr.w & 0xFF00u) != 0 || mr.y != 0;
+            const bool wk = busy >> q & 1u;
             if (wk) work |= 1u << q;
             if (L) {
               pings += d.P < L ? d.P : L;
@@ -873,21 +891,9 @@ __device__ __forceinline__ void scan_pass(const SimDev &d, uint32_t round, uint3
             risky |= 1u << q;
           }
         }
-      if (nstaged) {
-        __syncwarp();
-        bool fails = false;
-        if ((uint32_t)lane < (nstaged < 32u ? nstaged : 32u)) {
-          const uint4 e = stage[lane];
-          uint32_t am1[1] = {e.x}, td1[1] = {e.y};
-          const uint4 x = target_block<W>(d, round, e.z >> 2);
-          fails = probe_fails<W>(d, am1, td1, (uint32_t)__popc(e.x), word_of(x, e.z & 3), 0u, round, e.z);
-          fself = e.z;
-        }
-        fb = __ballot_sync(kFull, fails);
-        __syncwarp(); // the buffer is free again (next trip of this loop, or the passes that follow the scan)
-      }
-      // ... and pass 2 takes the others one per lane and trip (Philox block, r-th-set-bit picks): a lane pays for its own
-      // risky nodes only, not — by divergence — for every risky node of the warp.
+      // Pass 2 takes the nodes that were not staged one per lane and trip (Philox block, r-th-set-bit picks): a lane pays
+      // for its own risky nodes only, not — by divergence — for every risky node of the warp. It runs ahead of the staged
+      // picks, which need none of the records: the records are dead by then, and the staged pass keeps its registers.
       while (risky) {
         const int q = __ffs(risky) - 1;
         risky &= risky - 1;
@@ -900,6 +906,20 @@ __device__ __forceinline__ void scan_pass(const SimDev &d, uint32_t round, uint3
         uint32_t ldraw = 0;
         if (d.loss_ppm) ldraw = word_of(philox4x32_10(make_uint4(round, g, P_LOSS0, 0), d.key0, d.key1), q & 3);
         if (probe_fails<W>(d, am1, td1, (uint32_t)__popc(am1[0]), word_of(x, q & 3), ldraw, round, self)) work |= 1u << q;
+      }
+      // ... and the staged nodes, up to 32 at once
+      if (nstaged) {
+        __syncwarp();
+        bool fails = false;
+        if ((uint32_t)lane < (nstaged < 32u ? nstaged : 32u)) {
+          const uint4 e = stage[lane];
+          uint32_t am1[1] = {e.x}, td1[1] = {e.y};
+          const uint4 x = target_block<W>(d, round, e.z >> 2);
+          fails = probe_fails<W>(d, am1, td1, (uint32_t)__popc(e.x), word_of(x, e.z & 3), 0u, round, e.z);
+          fself = e.z;
+        }
+        fb = __ballot_sync(kFull, fails);
+        __syncwarp(); // the buffer is free again (next trip of this loop, or the passes that follow the scan)
       }
     } else {
 #pragma unroll
@@ -1018,8 +1038,9 @@ __device__ __forceinline__ uint32_t first_work_entry(const SimDev &d, uint32_t r
 // and a piggyback buffer that are already loaded (registers / the warp's shared-memory stage): work_pass walks the work
 // list with it; round_kernel_x also runs it right behind a node's mail. Lane s owns view slot s. Everything K1a derived is
 // recomputed from the row with warp ballots. Stores the row and the buffer; idx = the node's position on the round's work
-// list (its recipient slots, for the datagram export).
-template <int W>
+// list (its recipient slots, for the datagram export). kSharded = false: a single-shard launch (d.world == 1), in which
+// every recipient is local and the peer-memory and exchange-bucket stores do not exist.
+template <int W, bool kSharded = true>
 __device__ __forceinline__ void work_body(const SimDev &d, uint32_t round, uint32_t ln, uint32_t idx, Row<W> &row, const uint32_t (&rix)[W],
                                           const uint32_t (&td)[W], PbStage &pbs, Ctr &c, int lane, bool &did_remote,
                                           uint32_t next_ln, bool have_next) {
@@ -1201,12 +1222,13 @@ __device__ __forceinline__ void work_body(const SimDev &d, uint32_t round, uint3
                     ((wb0 >> (pb0 & 31) & 1u) && (wb1 >> (pb1 & 31) & 1u));
         }
       }
-      const uint32_t owner = d.world == 1 ? 0u : dst / d.per;
+      const uint32_t owner = (!kSharded || d.world == 1) ? 0u : dst / d.per;
       const uint32_t dl = dst - owner * d.per;
-      if (owner == d.rank) cand.x = dl | (deliver ? 0u : 0x80000000u); // bit 31: sent, nothing for K2 to do
+      const bool local = !kSharded || owner == d.rank;
+      if (local) cand.x = dl | (deliver ? 0u : 0x80000000u); // bit 31: sent, nothing for K2 to do
       if (!deliver) {
         // dropped at the sender
-      } else if (owner == d.rank) {
+      } else if (local) {
         d.eflag[(size_t)par * d.estride + ridx] = 1; // raise the in-edge flag (i -> dst)
         if (d.fused) atomicOr(&d.mailbits[(size_t)(round % 3u) * d.mbw + (dl >> 5)], 1u << (dl & 31));
       } else if (d.p2p) {
@@ -1245,12 +1267,14 @@ __device__ __forceinline__ void work_body(const SimDev &d, uint32_t round, uint3
     uint4 mine = make_uint4(0, 0, 0, 0);
     const bool have = (uint32_t)lane < pbs.cnt;
     if (have) { mine = pbs.s[lane]; d.out[((size_t)par * d.per + ln) * d.B + lane] = mine; }
-    unsigned xm = __ballot_sync(kFull, xs != 0xFFFFFFFFu);
-    while (xm) { // cross-shard envelopes carry the records themselves (staged NCCL path)
-      const int f = __ffs(xm) - 1;
-      xm &= xm - 1;
-      const uint32_t xslot = __shfl_sync(kFull, xs, f);
-      if (have) d.xsend[(size_t)xslot * (1 + d.B) + 1 + lane] = mine;
+    if (kSharded) {
+      unsigned xm = __ballot_sync(kFull, xs != 0xFFFFFFFFu);
+      while (xm) { // cross-shard envelopes carry the records themselves (staged NCCL path)
+        const int f = __ffs(xm) - 1;
+        xm &= xm - 1;
+        const uint32_t xslot = __shfl_sync(kFull, xs, f);
+        if (have) d.xsend[(size_t)xslot * (1 + d.B) + 1 + lane] = mine;
+      }
     }
     const bool keep = have && rec_ttl(mine) > 1;
     const unsigned km = __ballot_sync(kFull, keep);
@@ -1268,7 +1292,7 @@ __device__ __forceinline__ void work_body(const SimDev &d, uint32_t round, uint3
 }
 
 // K1b — warp-per-node over the work list.
-template <int W>
+template <int W, bool kSharded = true>
 __device__ __forceinline__ bool work_pass(const SimDev &d, uint32_t round, uint32_t warp, uint32_t nwarps, int lane,
                                           PbStage &pbs, Ctr &c, uint32_t first_ln, bool fence_remote = true) {
   const uint32_t n_work = d.wl_cnt[ci(round)];
@@ -1291,7 +1315,7 @@ __device__ __forceinline__ bool work_pass(const SimDev &d, uint32_t round, uint3
       rix[w] = W <= 2 ? d.ridx[(size_t)ln * d.cap + w * 32 + lane] : 0u;
       td[w] = d.meta[(size_t)ln * W + w].z;
     }
-    work_body<W>(d, round, ln, idx, row, rix, td, pbs, c, lane, did_remote, next_ln, have_next);
+    work_body<W, kSharded>(d, round, ln, idx, row, rix, td, pbs, c, lane, did_remote, next_ln, have_next);
   }
   if (did_remote && fence_remote) __threadfence_system(); // peer-memory stores are performed before the grid reports completion
   return did_remote;
@@ -1458,8 +1482,8 @@ __device__ __forceinline__ void recv_one(const SimDev &d, uint32_t round, uint32
 // Warp-per-receiver walk over the receivers of `round`, f(ln, early, snd) for each: the compact list of delivered slots
 // K1b wrote (early = true: the slot names one sender, snd, whose snapshot can be fetched with the row), then one list per
 // source rank (cross-shard senders). A receiver can be listed more than once: the claim stamp lets exactly one warp
-// process it.
-template <typename F>
+// process it. kSharded = false: a single-shard launch, which has no per-source-rank lists.
+template <bool kSharded = true, typename F>
 __device__ __forceinline__ void for_each_receiver(const SimDev &d, uint32_t round, uint32_t warp, uint32_t nwarps, F f) {
   const uint32_t par = round & 1;
   // items go to the warps from the top down: in the fused kernels the walk shares a phase with the scan, whose node ranges
@@ -1477,7 +1501,7 @@ __device__ __forceinline__ void for_each_receiver(const SimDev &d, uint32_t roun
     const uint2 e = item == w0 ? e_first : cl_in[item];
     f(e.x, true, e.y);
   }
-  if (d.world > 1) {
+  if (kSharded && d.world > 1) {
     uint32_t seg_end[SWIM_MAX_WORLD + 1];
     uint32_t n_recv = 0;
     seg_end[0] = 0;
@@ -1493,10 +1517,10 @@ __device__ __forceinline__ void for_each_receiver(const SimDev &d, uint32_t roun
   }
 }
 
-template <int W>
+template <int W, bool kSharded = true>
 __device__ __forceinline__ void recv_pass(const SimDev &d, uint32_t round, uint32_t warp, uint32_t nwarps,
                                           int lane, PbStage &pbs, Ctr &c, uint32_t tick_round = 0) {
-  for_each_receiver(d, round, warp, nwarps, [&](uint32_t ln, bool early, uint32_t snd) {
+  for_each_receiver<kSharded>(d, round, warp, nwarps, [&](uint32_t ln, bool early, uint32_t snd) {
     recv_one<W>(d, round, ln, early, snd, lane, pbs, c, tick_round);
   });
 }
@@ -1617,7 +1641,9 @@ __device__ __forceinline__ void clear_bitmap(const SimDev &d, uint32_t *bits, ui
   for (uint32_t x = warp * 32 + lane; x < d.mbw; x += nwarps * 32) bits[x] = 0;
 }
 
-template <int W>
+// kSharded: the launch is one shard of a multi-GPU run with the fused peer-memory exchange (d.world > 1 && d.p2p); the
+// single-shard instance has no handshake, no per-source-rank receive lists and no peer stores.
+template <int W, bool kSharded>
 __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel(SimDev d) {
   SWIM_SHARED_2D(uint4, s_pb, kWarpsPerBlock, 32);
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
@@ -1640,7 +1666,6 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel(SimDev d) {
   // into qm[batch % 3]; a slot is cleared two batches (>= two barriers) before it is used again, slot 0 here, ahead of the
   // first round's barrier. While rounds are quiet all three list counters stay zero, so the ordinary path resumes at any round.
   const bool batching = d.qbatch > 1 && d.world == 1 && d.loss_ppm == 0;
-  const bool sharded = d.world > 1 && d.p2p;
   bool prev_quiet = false, mail = false; // mail: round - 1 delivered envelopes to nodes of this rank
   uint32_t nb = 0;
   if (batching && warp == 0 && lane == 0) d.qm[0] = 0;
@@ -1672,7 +1697,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel(SimDev d) {
     // ---- phase S
     const uint32_t *skip = nullptr;
     if (mail) {
-      recv_pass<W>(d, round - 1, warp, nwarps, lane, pbs, c, round);     // K2 of the round before + those nodes' tick decision
+      recv_pass<W, kSharded>(d, round - 1, warp, nwarps, lane, pbs, c, round); // K2 of the round before + those nodes' tick decision
       skip = d.mailbits + (size_t)((round - 1) % 3u) * d.mbw;
     }
     uint32_t pings = 0;
@@ -1682,7 +1707,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel(SimDev d) {
     const uint32_t *wl_cnt_r = d.wl_cnt + ci(round);
     // the work list is complete. Sharded: a rank that listed nothing has no K1b to run, so its cross-GPU handshake of the
     // round happens right here, inside this barrier (one barrier for a quiet round)
-    if (sharded) grid_barrier<true>(d, round, 5, nullptr, nullptr, false, [&] { return *(volatile const uint32_t *)wl_cnt_r == 0; });
+    if constexpr (kSharded) grid_barrier<true>(d, round, 5, nullptr, nullptr, false, [&] { return *(volatile const uint32_t *)wl_cnt_r == 0; });
     else grid_barrier(d, round, 5);
     tl_mark(d, round, 2);
     const uint32_t n_work = d.wl_cnt[ci(round)];
@@ -1692,10 +1717,10 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel(SimDev d) {
     prev_quiet = n_work == 0 && !mail;
     // ---- phase W
     if (n_work) {
-      const bool remote = work_pass<W>(d, round, warp, nwarps, lane, pbs, c, first_ln, false); // K1b
+      const bool remote = work_pass<W, kSharded>(d, round, warp, nwarps, lane, pbs, c, first_ln, false); // K1b
       tl_mark(d, round, 3);
       // every flag and snapshot is written; sharded: ... on every rank (the last CTA talks to the peers)
-      if (sharded) grid_barrier<true>(d, round, 6, nullptr, nullptr, cta_or(remote));
+      if constexpr (kSharded) grid_barrier<true>(d, round, 6, nullptr, nullptr, cta_or(remote));
       else grid_barrier(d, round, 6);
       tl_mark(d, round, 4);
     }
@@ -1703,14 +1728,14 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel(SimDev d) {
     // the scan of round + 3 — both behind the next round's barriers, on this rank and, through the handshake, on its peers)
     // Was anything delivered here in this round? (every envelope dropped at its sender, or nobody sent: no)
     uint32_t got = n_work ? *(volatile uint32_t *)&d.ncand[ci(round)] : 0u;
-    if (sharded)
+    if (kSharded)
       for (uint32_t a = 0; a < d.world; ++a)
         if (a != d.rank) got |= *(volatile uint32_t *)&d.rcnt[(round & 1) * d.world + a];
     mail = got != 0;
     if (mail) prev_quiet = false;
   }
   if (mail) { // the last round's mail, before the launch ends (no tick decision: the next launch scans everybody)
-    recv_pass<W>(d, d.round + d.nrounds - 1, warp, nwarps, lane, pbs, c, 0);
+    recv_pass<W, kSharded>(d, d.round + d.nrounds - 1, warp, nwarps, lane, pbs, c, 0);
     // its bitmap is not needed by anybody: clear it. (The receive pass does not read it, so no barrier in between.)
     clear_bitmap(d, d.mailbits + (size_t)((d.round + d.nrounds - 1) % 3u) * d.mbw, warp, nwarps, lane);
   }
@@ -1735,7 +1760,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel(SimDev d) {
 // One node of the interval of round `round` (see above). from_wl: the node is item `idx` of the round's work list; else it
 // is a receiver of round - 1 named by a delivered slot (early / snd as in recv_one). mail: round - 1 delivered mail to
 // nodes of this rank at all. decide: take the tick decision of round + 1 (false in the last round of a launch).
-template <int W>
+template <int W, bool kSharded>
 __device__ __forceinline__ void x_node(const SimDev &d, uint32_t round, uint32_t ln, uint32_t idx, bool from_wl, bool mail, bool early,
                                        uint32_t snd, int lane, PbStage &pbs, Ctr &c, bool decide, bool &did_remote,
                                        uint32_t next_ln, bool have_next) {
@@ -1814,12 +1839,12 @@ __device__ __forceinline__ void x_node(const SimDev &d, uint32_t round, uint32_t
       }
     }
   }
-  if (do_work) work_body<W>(d, round, ln, idx, row, rix, td, pbs, c, lane, did_remote, next_ln, have_next);
+  if (do_work) work_body<W, kSharded>(d, round, ln, idx, row, rix, td, pbs, c, lane, did_remote, next_ln, have_next);
   else pb_store(pbs, d, ln, lane);
   if (decide) tick_decide<W>(d, round + 1, ln, row, pbs.cnt, td, lane, c, d.workbits + (size_t)((round + 1) % 3u) * d.mbw);
 }
 
-template <int W>
+template <int W, bool kSharded> // (kSharded: as for round_kernel)
 __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d) {
   SWIM_SHARED_2D(uint4, s_pb, kWarpsPerBlock, 32);
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
@@ -1830,7 +1855,6 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d)
   Ctr c; c.clear();
   PbStage pbs; pbs.s = s_pb[wib];
   const bool batching = d.qbatch > 1 && d.world == 1 && d.loss_ppm == 0;
-  const bool sharded = d.world > 1 && d.p2p;
   const uint32_t last_round = d.round + d.nrounds - 1;
   bool mail = false;       // round - 1 delivered envelopes to nodes of this rank
   bool have_wl = false;    // the work list of `round` exists (its length frozen in wl_n)
@@ -1897,9 +1921,9 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d)
       const uint2 *cl_in = d.cl + (size_t)mpar * d.n * d.fanout;
       for (uint32_t item = w0; item < n_cl; item += nwarps) {
         const uint2 e = cl_in[item];
-        x_node<W>(d, round, e.x, 0u, false, true, true, e.y, lane, pbs, c, !last, did_remote, 0u, false);
+        x_node<W, kSharded>(d, round, e.x, 0u, false, true, true, e.y, lane, pbs, c, !last, did_remote, 0u, false);
       }
-      if (d.world > 1) {
+      if (kSharded) {
         uint32_t seg_end[SWIM_MAX_WORLD + 1];
         uint32_t n_recv = 0;
         seg_end[0] = 0;
@@ -1911,7 +1935,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d)
           uint32_t a = 0;
           while (item >= seg_end[1 + a]) ++a;
           const uint32_t ln = d.rlr[((size_t)mpar * d.world + a) * d.rcap + (item - seg_end[a])];
-          x_node<W>(d, round, ln, 0u, false, true, false, 0u, lane, pbs, c, !last, did_remote, 0u, false);
+          x_node<W, kSharded>(d, round, ln, 0u, false, true, false, 0u, lane, pbs, c, !last, did_remote, 0u, false);
         }
       }
     }
@@ -1922,7 +1946,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d)
         const uint32_t ln = next_ln;
         const bool have_next = idx + nwarps < n_work;
         if (have_next) next_ln = *(volatile const uint32_t *)(wl + idx + nwarps);
-        x_node<W>(d, round, ln, idx, true, mail, false, 0u, lane, pbs, c, !last, did_remote, next_ln, have_next);
+        x_node<W, kSharded>(d, round, ln, idx, true, mail, false, 0u, lane, pbs, c, !last, did_remote, next_ln, have_next);
       }
     }
     if (!last) { // K1a of round + 1 for everybody else
@@ -1933,7 +1957,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d)
     }
     tl_mark(d, round, 1);
     // every flag, snapshot and list entry of the round is written (sharded: ... on every rank — the last CTA talks to the peers)
-    if (sharded) grid_barrier<true>(d, round, 5, d.wl_cnt + ci(round + 1), d.wl_n + ci(round + 1), cta_or(did_remote));
+    if constexpr (kSharded) grid_barrier<true>(d, round, 5, d.wl_cnt + ci(round + 1), d.wl_n + ci(round + 1), cta_or(did_remote));
     else grid_barrier(d, round, 5, d.wl_cnt + ci(round + 1), d.wl_n + ci(round + 1));
     tl_mark(d, round, 2);
     tl_mark(d, round, 4, (unsigned long long)(n_work || mail)); // 1: a busy round (bench.py tells busy from quiet rounds by it)
@@ -1941,14 +1965,14 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d)
     wb_prev = n_work != 0;
     // was anything delivered here in this round?
     uint32_t got = *(volatile uint32_t *)&d.ncand[ci(round)];
-    if (sharded)
+    if (kSharded)
       for (uint32_t a = 0; a < d.world; ++a)
         if (a != d.rank) got |= *(volatile uint32_t *)&d.rcnt[(round & 1) * d.world + a];
     mail = got != 0;
     known_empty = false;
   }
   // the last round's mail, before the launch ends (no tick decision: the next launch scans everybody)
-  if (mail) recv_pass<W>(d, last_round, warp, nwarps, lane, pbs, c, 0);
+  if (mail) recv_pass<W, kSharded>(d, last_round, warp, nwarps, lane, pbs, c, 0);
   // bitmaps still set: the mail of the last two rounds and the work lists (this rank's own affair: all three slots). Never
   // the mail slot of last + 1: a peer that is already in its next launch may be marking receivers there.
   clear_bitmap(d, d.mailbits + (size_t)(last_round % 3u) * d.mbw, warp, nwarps, lane);

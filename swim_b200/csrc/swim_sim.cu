@@ -553,8 +553,9 @@ static void prepare_kernels(swim_sim *sim) {
   sim->grids[0] = wave_grid(sim, tick_scan_kernel<W>, ((size_t)d.n + 128 * kScanGroups) / (128 * kScanGroups) + 1);
   sim->grids[1] = wave_grid(sim, tick_work_kernel<W>, (size_t)d.n);
   sim->grids[2] = wave_grid(sim, recv_kernel<W>, (size_t)d.n);
-  sim->grids[4] = wave_grid(sim, round_kernel<W>, (size_t)d.n);
-  sim->grids[5] = wave_grid(sim, round_kernel_x<W>, (size_t)d.n);
+  // (both instances of a round kernel: the grid must be co-resident whichever one a launch takes)
+  sim->grids[4] = std::min(wave_grid(sim, round_kernel<W, false>, (size_t)d.n), wave_grid(sim, round_kernel<W, true>, (size_t)d.n));
+  sim->grids[5] = std::min(wave_grid(sim, round_kernel_x<W, false>, (size_t)d.n), wave_grid(sim, round_kernel_x<W, true>, (size_t)d.n));
 #ifndef SWIM_EMU
   cudaFuncAttributes a;
   cudaFuncGetAttributes(&a, event_kernel<W>);
@@ -685,12 +686,13 @@ static int run_rounds(swim_sim *sim, uint32_t rounds) {
       // shard; SWIM_XMODE=1 / 0 forces it on (sharded runs included) / off.
       constexpr uint32_t kXModeMinRounds = 32;
       const bool use_x = sim->opt_xmode == 1 || (sim->opt_xmode < 0 && d.world == 1 && nr >= kXModeMinRounds);
+      const bool sharded = d.world > 1 && d.p2p; // (otherwise a single shard: single_kernel rules out the staged exchange)
       if (use_x) {
         d.xmode = 1;
-        CUDA_TRY(sim, launch_pdl(round_kernel_x<W>, sim->grids[5], sim->stream, d));
+        CUDA_TRY(sim, launch_pdl(sharded ? round_kernel_x<W, true> : round_kernel_x<W, false>, sim->grids[5], sim->stream, d));
         d.xmode = 0;
       } else {
-        CUDA_TRY(sim, launch_pdl(round_kernel<W>, kgrid, sim->stream, d));
+        CUDA_TRY(sim, launch_pdl(sharded ? round_kernel<W, true> : round_kernel<W, false>, kgrid, sim->stream, d));
       }
       d.fused = 0;
       ++sim->launches;
