@@ -103,12 +103,11 @@ struct SimDev {
   uint32_t *obs_off;         // [N+1] observers of member m among this shard's rows ...
   uint32_t *obs_slot;        // [n*cap] ... as linear slot indices l*cap + s
   uint32_t *wl, *wl_cnt;     // work lists of K1b [2][n] (round parity); counters indexed by round % 3
-  // one-barrier round kernel (round_kernel_x, `xmode`): a round's work list is still being extended (by the nodes whose mail
+  // one-barrier round kernel (round_kernel_x): a round's work list is still being extended (by the nodes whose mail
   // made them need K1b after all) while its items are walked, so the barrier that completes the list freezes its length in
   // wl_n[round % 3]; workbits: bit l of slot r % 3 = local node l is on the work list of round r
   uint32_t *wl_n;            // [3]
   uint32_t *workbits;        // [3][mbw]
-  uint32_t xmode;
   uint2 *rl;                 // [2][n*fanout] recipient slots (round parity), slot = item*fanout + f:
                              //   .x = local receiver (bit 31 set: sent, but not delivered — see `bloom`), .y = the sender
   // Mail bitmap (fused kernel only, `fused` != 0): bit l of slot (r % 3) = local node l was delivered mail in round r.
@@ -120,7 +119,7 @@ struct SimDev {
   uint32_t *mailbits;        // [3][mbw]
   uint32_t *mailbits_p[SWIM_MAX_WORLD];
   uint32_t mbw;              // words per parity = ceil(per / 32), the same on every rank
-  uint32_t fused;            // this launch is round_kernel (senders mark their receivers in the mail bitmap)
+  uint32_t fused;            // this launch is round_kernel or round_kernel_x (senders mark their receivers in the mail bitmap)
   uint2 *cl;                 // [2][n*fanout] the delivered slots of a round, compact (what K2 walks): {receiver, sender}
   uint32_t *ncand;           // [3] (round % 3) length of this round's compact list
   // Static membership filter of every node's view row (all N nodes, replicated on every rank): 512 W bits per node, two
@@ -707,7 +706,8 @@ __device__ __forceinline__ bool probe_fails(const SimDev &d, uint32_t (&am)[W], 
 // a draw selects, the Ack comes back, so the picks and the Philox blocks behind them are not needed — the common case.
 // The rule is stated from a node's meta words by node_needs_work (the wide-row scan, the batched quiet scan and, with the
 // draws made early, the receive pass) and from a view row a warp has loaded by tick_decide and x_node; the W == 1 scan
-// restates it inline. Each form is written for the register budget of the kernels it sits in.
+// restates it inline. Each form is written for the register budget of the kernels it sits in: one shared row form, used by
+// recv_one and x_node too, made ptxas spill more in several round-kernel instances (DESIGN.md §5).
 
 // From the meta words; counts the node's Pings as well.
 template <int W>
@@ -1641,6 +1641,40 @@ __device__ __forceinline__ void clear_bitmap(const SimDev &d, uint32_t *bits, ui
   for (uint32_t x = warp * 32 + lane; x < d.mbw; x += nwarps * 32) bits[x] = 0;
 }
 
+// One batched quiet scan of the Q rounds first .. first+Q-1 (quiet_scan) and its grid barrier, in the interval of `round`:
+// returns fb, the number of leading rounds that are quiet, and counts their Pings. The busy masks of the warps are OR-ed
+// into qm[nb % 3]; slot (nb + 1) % 3 is cleared for the next batch, two barriers ahead of its use (the caller clears slot
+// 0 before the first).
+template <int W>
+__device__ __forceinline__ uint32_t quiet_batch(const SimDev &d, uint32_t round, uint32_t first, uint32_t Q, uint32_t &nb,
+                                                uint32_t warp, uint32_t nwarps, int lane, Ctr &c) {
+  if (warp == 0 && lane == 0) d.qm[(nb + 1) % 3] = 0;
+  uint32_t p1 = 0;
+  uint32_t busy = quiet_scan<W>(d, first, Q, warp, nwarps, lane, p1);
+  busy = __reduce_or_sync(kFull, busy);
+  if (lane == 0 && busy) atomicOr(&d.qm[nb % 3], busy);
+  tl_mark(d, round, 1);
+  grid_barrier(d, round, 5);
+  const uint32_t mask = *(volatile uint32_t *)&d.qm[nb % 3];
+  ++nb;
+  const uint32_t fb = mask ? (uint32_t)__ffs(mask) - 1u : Q;
+  tl_mark(d, round, 2);
+  c.v[SWIM_CTR_PINGS] += p1 * fb;
+  return fb;
+}
+
+// Was mail of `round` delivered to nodes of this rank (behind the barrier that ends the round's K1b)? The length of the
+// round's compact list of local deliveries — zero if nobody sent: the slot is cleared before the round starts — and,
+// kSharded, the peers' counts of the receivers they listed here.
+template <bool kSharded>
+__device__ __forceinline__ bool mail_arrived(const SimDev &d, uint32_t round) {
+  uint32_t got = *(volatile uint32_t *)&d.ncand[ci(round)];
+  if (kSharded)
+    for (uint32_t a = 0; a < d.world; ++a)
+      if (a != d.rank) got |= *(volatile uint32_t *)&d.rcnt[(round & 1) * d.world + a];
+  return got != 0;
+}
+
 // kSharded: the launch is one shard of a multi-GPU run with the fused peer-memory exchange (d.world > 1 && d.p2p); the
 // single-shard instance has no handshake, no per-source-rank receive lists and no peer stores.
 template <int W, bool kSharded>
@@ -1677,19 +1711,8 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel(SimDev d) {
     if (warp == 0 && lane == 0) { d.wl_cnt[ci(round + 1)] = 0; d.ncand[ci(round + 1)] = 0; }
     if (batching && prev_quiet && d.nrounds - it >= 2) {
       const uint32_t Q = d.qbatch < d.nrounds - it ? d.qbatch : d.nrounds - it;
-      if (warp == 0 && lane == 0) d.qm[(nb + 1) % 3] = 0;
-      uint32_t p1 = 0;
-      uint32_t busy = quiet_scan<W>(d, round, Q, warp, nwarps, lane, p1);
-      busy = __reduce_or_sync(kFull, busy);
-      if (lane == 0 && busy) atomicOr(&d.qm[nb % 3], busy);
-      tl_mark(d, round, 1);
-      grid_barrier(d, round, 5);
-      const uint32_t mask = *(volatile uint32_t *)&d.qm[nb % 3];
-      ++nb;
-      const uint32_t fb = mask ? (uint32_t)__ffs(mask) - 1u : Q; // rounds round .. round+fb-1 are quiet: committed
-      tl_mark(d, round, 2);
+      const uint32_t fb = quiet_batch<W>(d, round, round, Q, nb, warp, nwarps, lane, c); // rounds round .. round+fb-1: committed
       tl_mark(d, round, 7, fb);
-      c.v[SWIM_CTR_PINGS] += p1 * fb;
       prev_quiet = fb == Q;
       if (fb) { it += fb - 1; continue; }
       // fb == 0: this very round has work — the ordinary scan below lists it
@@ -1727,11 +1750,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel(SimDev d) {
     // (no barrier is owed to the bitmap clear: that slot is written again by the senders of round + 2 and read again by
     // the scan of round + 3 — both behind the next round's barriers, on this rank and, through the handshake, on its peers)
     // Was anything delivered here in this round? (every envelope dropped at its sender, or nobody sent: no)
-    uint32_t got = n_work ? *(volatile uint32_t *)&d.ncand[ci(round)] : 0u;
-    if (kSharded)
-      for (uint32_t a = 0; a < d.world; ++a)
-        if (a != d.rank) got |= *(volatile uint32_t *)&d.rcnt[(round & 1) * d.world + a];
-    mail = got != 0;
+    mail = mail_arrived<kSharded>(d, round);
     if (mail) prev_quiet = false;
   }
   if (mail) { // the last round's mail, before the launch ends (no tick decision: the next launch scans everybody)
@@ -1887,22 +1906,9 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d)
       // `round` is quiet — nothing to apply, nothing to run — and so committed. One pass decides rounds round+1 .. round+Q.
       // (No list is appended to and no mail counted while rounds are quiet: all counters of the three slots are cleared.)
       const uint32_t Q = d.qbatch < last_round - round ? d.qbatch : last_round - round;
-      if (warp == 0 && lane == 0) {
-        d.qm[(nb + 1) % 3] = 0;
-        d.wl_cnt[ci(round + 1)] = 0; d.wl_cnt[ci(round + 2)] = 0; d.ncand[ci(round + 1)] = 0;
-      }
-      uint32_t p1 = 0;
-      uint32_t busy = quiet_scan<W>(d, round + 1, Q, warp, nwarps, lane, p1);
-      busy = __reduce_or_sync(kFull, busy);
-      if (lane == 0 && busy) atomicOr(&d.qm[nb % 3], busy);
-      tl_mark(d, round, 1);
-      grid_barrier(d, round, 5);
-      const uint32_t mask = *(volatile uint32_t *)&d.qm[nb % 3];
-      ++nb;
-      const uint32_t fb = mask ? (uint32_t)__ffs(mask) - 1u : Q; // rounds round+1 .. round+fb are quiet too
-      tl_mark(d, round, 2);
+      if (warp == 0 && lane == 0) { d.wl_cnt[ci(round + 1)] = 0; d.wl_cnt[ci(round + 2)] = 0; d.ncand[ci(round + 1)] = 0; }
+      const uint32_t fb = quiet_batch<W>(d, round, round + 1, Q, nb, warp, nwarps, lane, c); // rounds round+1 .. round+fb are quiet too
       tl_mark(d, round, 7, fb == Q ? Q : fb + 1); // rounds committed by this pass
-      c.v[SWIM_CTR_PINGS] += p1 * fb;
       // fb == Q: round+Q is decided (quiet) but not yet committed: it is the next current round, with a list known to be
       // empty. fb < Q: round+fb+1 is busy: it gets the ordinary scan above.
       if (fb == Q) { it += Q - 1; known_empty = true; }
@@ -1963,12 +1969,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d)
     tl_mark(d, round, 4, (unsigned long long)(n_work || mail)); // 1: a busy round (bench.py tells busy from quiet rounds by it)
     mail_prev = mail;
     wb_prev = n_work != 0;
-    // was anything delivered here in this round?
-    uint32_t got = *(volatile uint32_t *)&d.ncand[ci(round)];
-    if (kSharded)
-      for (uint32_t a = 0; a < d.world; ++a)
-        if (a != d.rank) got |= *(volatile uint32_t *)&d.rcnt[(round & 1) * d.world + a];
-    mail = got != 0;
+    mail = mail_arrived<kSharded>(d, round);
     known_empty = false;
   }
   // the last round's mail, before the launch ends (no tick decision: the next launch scans everybody)

@@ -687,13 +687,10 @@ static int run_rounds(swim_sim *sim, uint32_t rounds) {
       constexpr uint32_t kXModeMinRounds = 32;
       const bool use_x = sim->opt_xmode == 1 || (sim->opt_xmode < 0 && d.world == 1 && nr >= kXModeMinRounds);
       const bool sharded = d.world > 1 && d.p2p; // (otherwise a single shard: single_kernel rules out the staged exchange)
-      if (use_x) {
-        d.xmode = 1;
+      if (use_x)
         CUDA_TRY(sim, launch_pdl(sharded ? round_kernel_x<W, true> : round_kernel_x<W, false>, sim->grids[5], sim->stream, d));
-        d.xmode = 0;
-      } else {
+      else
         CUDA_TRY(sim, launch_pdl(sharded ? round_kernel<W, true> : round_kernel<W, false>, kgrid, sim->stream, d));
-      }
       d.fused = 0;
       ++sim->launches;
       sim->round += nr - 1;
