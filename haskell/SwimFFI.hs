@@ -18,6 +18,8 @@ module SwimFFI
     -- raw imports of the bulk / codec / replay entry points (marshalled by the caller)
   , c_simSetRound, c_simSave, c_simLoad, c_simSetParams, c_simInject, c_simGetArray, c_simSetArray, c_simCounters, c_simObserve, c_simExportRound
   , c_simInjectDatagram, c_getBroadcasts, c_takeBroadcasts, c_tickTimers, c_envEncode, c_envDecode, simCounters
+    -- bulk membership edits between steps: removeDeadNodes / addNewMember on every store at once
+  , c_simRemoveDeadNodes, c_simAddMembers
   ) where
 
 import Control.Monad (when)
@@ -138,6 +140,10 @@ foreign import ccall safe   "swim_sim_inject_datagram" c_simInjectDatagram :: Si
 foreign import ccall safe   "swim_get_broadcasts"      c_getBroadcasts     :: Sim -> Word32 -> Ptr CMessage -> CSize -> Ptr CSize -> IO CInt
 foreign import ccall safe   "swim_take_broadcasts"     c_takeBroadcasts    :: Sim -> Word32 -> Ptr CMessage -> CSize -> Ptr CSize -> IO CInt
 foreign import ccall safe   "swim_tick_timers"         c_tickTimers        :: Sim -> Word32 -> Ptr Word32 -> IO CInt
+-- removeDeadNodes (Core.hs:65-67) with a minimum age, and addNewMember (Core.hs:206-216) over an array of
+-- swim_member_add_t {observer, member, incarnation, _pad :: Word32}; single shard, between steps
+foreign import ccall safe   "swim_sim_remove_dead_nodes" c_simRemoveDeadNodes :: Sim -> Word32 -> Ptr Word64 -> IO CInt
+foreign import ccall safe   "swim_sim_add_members"     c_simAddMembers     :: Sim -> Ptr Word32 -> CSize -> Ptr Word64 -> Ptr Word64 -> IO CInt
 foreign import ccall unsafe "swim_envelope_encode"     c_envEncode         :: Ptr () -> CSize -> Ptr Word8 -> CSize -> Ptr CSize -> IO CInt
 foreign import ccall unsafe "swim_envelope_decode"     c_envDecode         :: Ptr Word8 -> CSize -> Ptr () -> CSize -> Ptr CSize -> IO CInt
 

@@ -249,6 +249,11 @@ int swim_sim_local_range(const swim_sim_t *sim, uint32_t *first, uint32_t *count
  * index of its own nodes. */
 int swim_sim_set_view(swim_sim_t *sim, const uint32_t *nbr_global);
 
+/* The same with the matrix already in device memory on the handle's device (read on the handle's stream): no host
+ * copy of the N * view_cap ids. Either call builds the in-edge index, the observer lists and the membership filters on
+ * the device. SWIM_ESTATE after swim_sim_ipc_connect, as for swim_sim_set_view. */
+int swim_sim_set_view_device(swim_sim_t *sim, const uint32_t *nbr_global_dev);
+
 /* Host-side synthetic topologies (BASELINE configs): rows of `degree` distinct ids != i.
  * kind 0 = complete (degree ignored, needs N-1 <= view_cap), 1 = uniform random,
  * 2 = ring lattice (i±1..±degree/2). out is [N*view_cap]. No device needed. */
@@ -289,7 +294,7 @@ int swim_sim_set_round(swim_sim_t *sim, uint32_t round);
  * events into a second set of device arrays: stream-ordered device-to-device copies, no host traffic. swim_sim_load puts
  * the handle back there (and clears every round-stamped scratch array), so the same rounds can be stepped again and
  * give the same result — what a parameter sweep or a repeated timing window needs. A new view (swim_sim_set_view) or
- * a membership change through the scalar calls drops the checkpoint. Sharded runs: every rank saves / loads its own
+ * a membership change through the scalar or bulk calls drops the checkpoint. Sharded runs: every rank saves / loads its own
  * shard while ALL ranks are between steps (host-side barrier before and after). */
 int swim_sim_save(swim_sim_t *sim);
 int swim_sim_load(swim_sim_t *sim);
@@ -299,6 +304,25 @@ int swim_sim_load(swim_sim_t *sim);
  * (SWIM_EINVAL otherwise: sizes and the shard layout are fixed at create). With swim_sim_save / swim_sim_load this is a
  * parameter sweep on ONE handle: the view, its in-edge index and the device arrays are built once. */
 int swim_sim_set_params(swim_sim_t *sim, const swim_config_t *cfg);
+
+/* Bulk membership edits between steps, on the device (one warp per affected row, no host copy of the rows). Single
+ * shard only (SWIM_ESTATE when world > 1). Both mark the view changed: the next step rebuilds the in-edge index, the
+ * checkpoint is dropped (swim_sim_load fails until the next swim_sim_save), and swim_sim_export_round returns
+ * SWIM_ESTATE until the next step.
+ *
+ * removeDeadNodes (Core.hs:65-67) on every local store at once: Dead entries with round - last_change >= min_age leave
+ * (round = rounds executed so far; min_age = 0 is the reference's form, swim_remove_dead_nodes on every node). Rows stay
+ * ascending with vacancies last. *n_removed (may be NULL) = entries removed. */
+int swim_sim_remove_dead_nodes(swim_sim_t *sim, uint32_t min_age, uint64_t *n_removed);
+
+/* addNewMember (Core.hs:206-216) for many stores, applied in the order given: a member the observer does not list is
+ * inserted as Alive with `incarnation` and last_change = the current round (what an inserting swim_alive_node does); a
+ * member it lists is left untouched; an add to a full row is dropped and counted in *n_full. Every add is checked
+ * before anything changes (ids < N, member != observer; SWIM_EINVAL otherwise). Outputs may be NULL. */
+typedef struct swim_member_add {
+  uint32_t observer, member, incarnation, _pad;
+} swim_member_add_t;
+int swim_sim_add_members(swim_sim_t *sim, const swim_member_add_t *adds, size_t n, uint64_t *n_added, uint64_t *n_full);
 
 /* Bulk copies of one state array (SWIM_ARR_*) between device and a host buffer of exactly
  * `bytes` bytes. set_array(SWIM_ARR_NBR) is rejected: use swim_sim_set_view. */

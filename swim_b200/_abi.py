@@ -69,6 +69,10 @@ class Event(C.Structure):
                 ("msg", Message)]
 
 
+class MemberAdd(C.Structure):
+    _fields_ = [("observer", C.c_uint32), ("member", C.c_uint32), ("incarnation", C.c_uint32), ("_pad", C.c_uint32)]
+
+
 class Datagram(C.Structure):
     _fields_ = [("src", C.c_uint32), ("dst", C.c_uint32), ("length", C.c_uint32), ("n_messages", C.c_uint32),
                 ("offset", C.c_uint64)]
@@ -90,6 +94,7 @@ EVENT_DTYPE = _np.dtype({"names": ["round", "node", "kind", "msg_kind", "msg_nod
                          "formats": ["<u4", "<u4", "u1", "u1", "<u4", "<i8", "<u4"],
                          "offsets": [0, 4, 8, 16, 24, 32, 40],
                          "itemsize": C.sizeof(Event)})
+MEMBER_ADD_DTYPE = _np.dtype([("observer", "<u4"), ("member", "<u4"), ("incarnation", "<u4"), ("_pad", "<u4")])
 ARRAY_DTYPES = {
     ARR_ALIVE: _np.dtype("u1"), ARR_SELF_INC: _np.dtype("<u4"), ARR_SEQNO: _np.dtype("<u4"),
     ARR_NBR: _np.dtype("<u4"), ARR_VST: _np.dtype("u1"), ARR_VINC: _np.dtype("<u4"),

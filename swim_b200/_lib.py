@@ -44,6 +44,9 @@ def lib():
     sig("swim_sim_destroy", None, vp)
     sig("swim_sim_local_range", i, vp, P(u32), P(u32))
     sig("swim_sim_set_view", i, vp, vp)
+    sig("swim_sim_set_view_device", i, vp, vp)
+    sig("swim_sim_remove_dead_nodes", i, vp, u32, P(u64))
+    sig("swim_sim_add_members", i, vp, vp, sz, P(u64), P(u64))
     sig("swim_topology_generate", i, i, u32, u32, u32, u64, vp)
     sig("swim_sim_set_round", i, vp, u32)
     sig("swim_sim_save", i, vp)

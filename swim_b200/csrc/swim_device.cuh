@@ -636,8 +636,8 @@ constexpr int kScanGroups = 2; // Philox groups (of 4 nodes) per lane per iterat
 __device__ __forceinline__ uint32_t ci(uint32_t round) { return round % 3u; } // slot of the per-round list counters
 __device__ __forceinline__ uint32_t *wl_of(const SimDev &d, uint32_t round) { return d.wl + (size_t)(round & 1u) * d.n; } // that round's work list
 
-// The two filter positions of member id x in a node's 512 W-bit membership filter (SimDev::bloom); the host builds the
-// filters with the same two lines (swim_sim.cu: build_in_edges).
+// The two filter positions of member id x in a node's 512 W-bit membership filter (SimDev::bloom); bloom_kernel
+// (swim_graph.cuh) builds the filters with the same two lines.
 SWIM_HD uint32_t bloom_pos(uint32_t x, int which, uint32_t bits) {
   return SWIM_UMULHI(x * (which ? 0x85EBCA77u : 0x9E3779B1u), bits);
 }

@@ -52,6 +52,7 @@ extern "C" int swim_sim_export_round(swim_sim_t *sim, uint8_t *buf, size_t cap, 
   if (!sim || !n_datagrams || !n_bytes) return SWIM_EINVAL;
   const SimDev &d = sim->dev;
   if (d.world != 1) { set_error(sim, "swim_sim_export_round: single shard only"); return SWIM_ESTATE; }
+  if (sim->rows_edited) { set_error(sim, "swim_sim_export_round: memberships were edited since the last step"); return SWIM_ESTATE; }
   *n_datagrams = 0;
   *n_bytes = 0;
   if (sim->round == 0) return SWIM_OK;

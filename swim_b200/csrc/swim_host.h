@@ -19,7 +19,8 @@ struct swim_sim {
   bool timed = false;
   uint32_t round = 0;
   bool view_set = false;
-  bool edges_dirty = false; // scalar calls changed a row's membership
+  bool edges_dirty = false; // scalar or bulk calls changed a row's membership: the mail graph is rebuilt by the next step
+  bool rows_edited = false; // a bulk membership edit since the last step: the last round's envelopes no longer match the rows
   bool tdead_dirty = true;  // crashed-member bitmaps must be rebuilt from alive[]
   bool connected = false;   // multi-shard exchange ready
   uint64_t n_edges = 0;
@@ -38,7 +39,7 @@ struct swim_sim {
   // device-resident checkpoint (swim_sim_save / swim_sim_load): one slot per handle
   std::vector<std::pair<void *, size_t>> ckpt_arrays; // (copy, bytes) in the order of ckpt_sources()
   uint32_t ckpt_round = 0;
-  uint64_t view_epoch = 0, ckpt_epoch = 0; // build_in_edges counts views; a checkpoint belongs to one
+  uint64_t view_epoch = 0, ckpt_epoch = 0; // build_graph (swim_graph.cuh) counts views; a checkpoint belongs to one
   bool ckpt_valid = false;
   std::vector<swim_event_t> ckpt_events;
   unsigned long long *d_scratch = nullptr;

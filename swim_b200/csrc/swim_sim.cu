@@ -3,9 +3,6 @@
 // conduits and a ticker thread per OS process, one handle owns N stores in HBM and
 // swim_sim_step runs the protocol period for all of them.
 #include <algorithm>
-#ifdef _OPENMP
-#include <omp.h>
-#endif
 #include <chrono>
 #include <cstdarg>
 #include <cstdio>
@@ -301,182 +298,8 @@ extern "C" int swim_sim_local_range(const swim_sim_t *sim, uint32_t *first, uint
   return SWIM_OK;
 }
 
-// Build the in-edge index of the local nodes from the global id matrix and upload it.
-// in-list of receiver j = senders i (ascending) that have j in their row; the flag of edge
-// (i -> j) lives at in_off[j] + position; ridx[i, s] is that position for local senders.
-static int build_in_edges(swim_sim *sim, const uint32_t *nbr) {
-  SimDev &d = sim->dev;
-  const uint32_t N = d.N, cap = d.cap;
-  // Both passes over the global matrix are partitioned by RECEIVER id: thread t owns the receivers of its id range, reads
-  // the whole matrix (sequential, cheap) and touches only its own slice of the per-receiver arrays (which then fits a
-  // cache), so there are no conflicts and the senders of a receiver are still met in ascending order. At 2^24 nodes the
-  // serial form of this function was most of swim_sim_set_view's 34 s.
-  int n_thr = 1;
-#ifdef _OPENMP
-  n_thr = std::max(1, omp_get_max_threads());
-#endif
-  const auto range_of = [&](int t) { return (uint32_t)(((uint64_t)N * (uint64_t)t) / (uint64_t)n_thr); };
-  // global in-degree, then per-shard exclusive offsets
-  std::vector<uint32_t> deg((size_t)N + 1, 0);
-  size_t bad_x = (size_t)-1;
-#pragma omp parallel num_threads(n_thr)
-  {
-#ifdef _OPENMP
-    const int t = omp_get_thread_num();
-#else
-    const int t = 0;
-#endif
-    const uint32_t j0 = range_of(t), j1 = range_of(t + 1);
-    for (size_t x = 0, tot = (size_t)N * cap; x < tot; ++x) {
-      const uint32_t j = nbr[x];
-      if (j - j0 < j1 - j0) deg[j]++;
-      else if (t == 0 && j >= N && j != SWIM_NO_MEMBER) bad_x = x; // rows of other shards are not validated by swim_sim_set_view
-    }
-  }
-  if (bad_x != (size_t)-1) {
-    set_error(sim, "view matrix entry %zu holds id %u >= N (%u)", bad_x, nbr[bad_x], N);
-    return SWIM_EINVAL;
-  }
-  std::vector<uint64_t> goff((size_t)N + 1);
-  uint64_t acc = 0;
-  for (uint32_t j = 0; j <= N; ++j) {
-    if (j % d.per == 0) acc = 0; // offsets restart at every shard boundary
-    goff[j] = acc;
-    if (j < N) acc += deg[j];
-  }
-  // goff[j] for j at a shard boundary is 0; the shard's edge count is needed separately
-  uint64_t E = 0;
-  for (uint32_t j = d.first; j < d.first + d.n; ++j) E += deg[j];
-  if (E > 0xFFFFFFFFull) { set_error(sim, "in-edge count %llu exceeds 2^32", (unsigned long long)E); return SWIM_ERANGE; }
-  std::vector<uint32_t> in_off((size_t)d.n + 1), in_src((size_t)E ? (size_t)E : 1), ridx((size_t)d.n * cap, 0);
-  for (uint32_t l = 0; l < d.n; ++l) in_off[l] = (uint32_t)goff[d.first + l];
-  in_off[d.n] = (uint32_t)E;
-  std::vector<uint32_t> &cursor = deg; // edges seen so far per receiver (the degrees are not needed any more)
-  std::fill(cursor.begin(), cursor.end(), 0u);
-#pragma omp parallel num_threads(n_thr)
-  {
-#ifdef _OPENMP
-    const int t = omp_get_thread_num();
-#else
-    const int t = 0;
-#endif
-    const uint32_t j0 = range_of(t), j1 = range_of(t + 1);
-    for (uint32_t i = 0; i < N; ++i) {
-      const bool mine = i >= d.first && i < d.first + d.n;
-      const uint32_t *row = nbr + (size_t)i * cap;
-      for (uint32_t s = 0; s < cap; ++s) {
-        const uint32_t j = row[s];
-        if (j - j0 >= j1 - j0) continue; // another thread's receiver (or a vacant slot)
-        const uint32_t pos = cursor[j]++;
-        if (j >= d.first && j < d.first + d.n) in_src[(size_t)goff[j] + pos] = i;
-        if (mine) ridx[(size_t)(i - d.first) * cap + s] = (uint32_t)goff[j] + pos;
-      }
-    }
-  }
-  // observers: for every member id m, the local slots (l*cap + s) that hold m — the transpose of
-  // the local rows, used to keep the crashed-member bitmaps current on crash / rejoin events
-  {
-    std::vector<uint32_t> obs_off((size_t)N + 1, 0), obs_slot((size_t)d.n * cap ? (size_t)d.n * cap : 1);
-    const uint32_t *rows = nbr + (size_t)d.first * cap;
-    for (size_t x = 0, tot = (size_t)d.n * cap; x < tot; ++x)
-      if (rows[x] != SWIM_NO_MEMBER) obs_off[rows[x] + 1]++;
-    for (uint32_t m = 0; m < N; ++m) obs_off[m + 1] += obs_off[m];
-    std::vector<uint32_t> cur(obs_off.begin(), obs_off.end() - 1);
-    for (size_t x = 0, tot = (size_t)d.n * cap; x < tot; ++x)
-      if (rows[x] != SWIM_NO_MEMBER) obs_slot[cur[rows[x]]++] = (uint32_t)x;
-    CUDA_TRY(sim, cudaMemcpy(d.obs_off, obs_off.data(), obs_off.size() * 4, cudaMemcpyHostToDevice));
-    CUDA_TRY(sim, cudaMemcpy(d.obs_slot, obs_slot.data(), (size_t)d.n * cap * 4, cudaMemcpyHostToDevice));
-  }
-  // membership filters of ALL rows (a sender tests its records against the recipient's filter, wherever the recipient
-  // lives): 16 * cap bits per node, two positions per member id (bloom_pos, shared with the device code)
-  {
-    const uint32_t bits = 16 * cap, words = bits / 32;
-    std::vector<uint32_t> bloom((size_t)N * words, 0u);
-#pragma omp parallel for schedule(static)
-    for (int64_t i = 0; i < (int64_t)N; ++i) {
-      uint32_t *bf = bloom.data() + (size_t)i * words;
-      for (uint32_t s = 0; s < cap; ++s) {
-        const uint32_t m = nbr[(size_t)i * cap + s];
-        if (m == SWIM_NO_MEMBER) continue;
-        for (int which = 0; which < 2; ++which) {
-          const uint32_t pos = bloom_pos(m, which, bits);
-          bf[pos >> 5] |= 1u << (pos & 31);
-        }
-      }
-    }
-    if (sim->d_bloom) { cudaFree(sim->d_bloom); sim->d_bloom = nullptr; }
-    CUDA_TRY(sim, cudaMalloc((void **)&sim->d_bloom, bloom.size() * 4));
-    CUDA_TRY(sim, cudaMemcpy(sim->d_bloom, bloom.data(), bloom.size() * 4, cudaMemcpyHostToDevice));
-    d.bloom = sim->d_bloom;
-  }
-  sim->tdead_dirty = true;
-  ++sim->view_epoch;
-  if (sim->d_in_src) { cudaFree(sim->d_in_src); sim->d_in_src = nullptr; }
-  if (sim->d_eflag) { cudaFree(sim->d_eflag); sim->d_eflag = nullptr; }
-  const size_t Ea = E ? (size_t)E : 1;
-  const size_t estride = (Ea + 255) & ~(size_t)255; // parity stride of the mail flags
-  d.estride = (uint32_t)estride;
-  CUDA_TRY(sim, cudaMalloc((void **)&sim->d_in_src, Ea * 4));
-  CUDA_TRY(sim, cudaMalloc((void **)&sim->d_eflag, 2 * estride));
-  CUDA_TRY(sim, cudaMemset(sim->d_eflag, 0, 2 * estride));
-  CUDA_TRY(sim, cudaMemcpy(sim->d_in_src, in_src.data(), Ea * 4, cudaMemcpyHostToDevice));
-  CUDA_TRY(sim, cudaMemcpy(d.in_off, in_off.data(), ((size_t)d.n + 1) * 4, cudaMemcpyHostToDevice));
-  CUDA_TRY(sim, cudaMemcpy(d.ridx, ridx.data(), ridx.size() * 4, cudaMemcpyHostToDevice));
-  d.in_src = sim->d_in_src;
-  d.eflag = sim->d_eflag;
-  sim->n_edges = E;
-  return swim::dist_alloc_edges(sim);
-}
-
-extern "C" int swim_sim_set_view(swim_sim_t *sim, const uint32_t *nbr) {
-  if (!sim || !nbr) return SWIM_EINVAL;
-  SimDev &d = sim->dev;
-  if (d.p2p) { set_error(sim, "swim_sim_set_view: peers already mapped this rank's arrays (set the view before swim_sim_ipc_connect)"); return SWIM_ESTATE; }
-  cudaSetDevice(sim->device);
-  CUDA_TRY(sim, cudaStreamSynchronize(sim->stream));
-  // validate the local rows: ascending, distinct, in range, never self, vacancies last
-  for (uint32_t l = 0; l < d.n; ++l) {
-    const uint32_t *row = nbr + (size_t)(d.first + l) * d.cap;
-    uint32_t prev = 0;
-    bool seen = false, vacant = false;
-    for (uint32_t s = 0; s < d.cap; ++s) {
-      const uint32_t m = row[s];
-      if (m == SWIM_NO_MEMBER) { vacant = true; continue; }
-      if (vacant || m >= d.N || m == d.first + l || (seen && m <= prev)) {
-        set_error(sim, "swim_sim_set_view: row %u slot %u is not a sorted set of ids != self", d.first + l, s);
-        return SWIM_EINVAL;
-      }
-      prev = m; seen = true;
-    }
-  }
-  const size_t slots = (size_t)d.n * d.cap;
-  std::vector<uint8_t> st(slots ? slots : 1);
-  const uint32_t *mine = nbr + (size_t)d.first * d.cap;
-  for (size_t x = 0; x < slots; ++x) st[x] = mine[x] == SWIM_NO_MEMBER ? SWIM_VACANT : SWIM_ALIVE;
-  CUDA_TRY(sim, cudaMemcpy(d.nbr, mine, slots * 4, cudaMemcpyHostToDevice));
-  CUDA_TRY(sim, cudaMemcpy(d.vst, st.data(), slots, cudaMemcpyHostToDevice));
-  CUDA_TRY(sim, cudaMemset(d.vinc, 0, slots * 4));
-  CUDA_TRY(sim, cudaMemset(d.vlast, 0, slots * 4));
-  int rc = build_in_edges(sim, nbr);
-  if (rc) return rc;
-  sim->view_set = true;
-  sim->edges_dirty = false;
-  return SWIM_OK;
-}
-
-// Rebuild the in-edge index from the device rows (after scalar calls changed memberships).
-namespace swim {
-int rebuild_edges_from_device(swim_sim *sim) {
-  SimDev &d = sim->dev;
-  if (d.world != 1) { set_error(sim, "view membership changes are single-shard only"); return SWIM_ESTATE; }
-  std::vector<uint32_t> nbr((size_t)d.N * d.cap);
-  CUDA_TRY(sim, cudaMemcpy(nbr.data(), d.nbr, nbr.size() * 4, cudaMemcpyDeviceToHost));
-  int rc = build_in_edges(sim, nbr.data());
-  if (rc) return rc;
-  sim->edges_dirty = false;
-  return SWIM_OK;
-}
-} // namespace swim
+// swim_sim_set_view / _set_view_device, the device-side mail-graph build and the bulk membership edits
+#include "swim_graph.cuh"
 
 // ------------------------------------------------------------------ events
 extern "C" int swim_sim_inject(swim_sim_t *sim, const swim_event_t *ev, size_t n) {
@@ -750,6 +573,7 @@ static int step_async_impl(swim_sim_t *sim, uint32_t rounds, bool timed) {
   if (rc) { sim->failed = true; return rc; } // rounds and events were consumed: no retry on this handle
   if (timed) CUDA_TRY(sim, cudaEventRecord(sim->ev_stop, sim->stream));
   sim->timed = timed;
+  sim->rows_edited = false;
   return SWIM_OK;
 }
 

@@ -116,10 +116,43 @@ class Simulator:
 
     # ---- bulk path
     def set_view(self, nbr):
+        """Install the view graph: the global [N, view_cap] id matrix, as a NumPy array or as a torch CUDA tensor (int32 or
+        uint32, contiguous, on the handle's device), which is read in place (swim_sim_set_view_device)."""
+        if getattr(nbr, "is_cuda", False):
+            import torch
+            if nbr.dtype not in (torch.int32, torch.uint32) or not nbr.is_contiguous():
+                raise ValueError("a CUDA view matrix must be a contiguous int32 or uint32 tensor")
+            if nbr.numel() != self.cfg.n_nodes * self.cfg.view_cap:
+                raise ValueError("nbr must be the global [N, view_cap] id matrix")
+            if self.cfg.device >= 0 and nbr.device.index != self.cfg.device:
+                raise ValueError(f"the view matrix is on {nbr.device}, the handle on cuda:{self.cfg.device}")
+            torch.cuda.current_stream(nbr.device).synchronize()  # the handle reads it on its own stream
+            check(lib().swim_sim_set_view_device(self._h, nbr.data_ptr()), "swim_sim_set_view_device", self._h)
+            return
         nbr = np.ascontiguousarray(nbr, dtype=np.uint32)
         if nbr.size != self.cfg.n_nodes * self.cfg.view_cap:
             raise ValueError("nbr must be the global [N, view_cap] id matrix")
         check(lib().swim_sim_set_view(self._h, nbr.ctypes.data), "swim_sim_set_view", self._h)
+
+    def remove_dead_nodes(self, min_age=0):
+        """removeDeadNodes (Core.hs:65-67) on every local store: Dead entries at least `min_age` rounds old leave.
+        Returns the number removed. Single shard; the next step rebuilds the mail graph."""
+        n = C.c_uint64()
+        check(lib().swim_sim_remove_dead_nodes(self._h, min_age, C.byref(n)), "swim_sim_remove_dead_nodes", self._h)
+        return n.value
+
+    def add_members(self, observers, members, incarnations=0):
+        """addNewMember (Core.hs:206-216) for many stores, in the order given: an unlisted member is inserted Alive with
+        its incarnation, a listed one is left alone, an add to a full row is dropped. Returns (added, full)."""
+        observers = np.atleast_1d(np.asarray(observers))
+        adds = np.zeros(len(observers), dtype=A.MEMBER_ADD_DTYPE)
+        adds["observer"] = observers
+        adds["member"] = members
+        adds["incarnation"] = incarnations
+        added, full = C.c_uint64(), C.c_uint64()
+        check(lib().swim_sim_add_members(self._h, adds.ctypes.data, len(adds), C.byref(added), C.byref(full)),
+              "swim_sim_add_members", self._h)
+        return added.value, full.value
 
     def inject(self, events):
         events = np.ascontiguousarray(events, dtype=A.EVENT_DTYPE)
