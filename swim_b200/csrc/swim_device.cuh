@@ -8,9 +8,10 @@
 //   K2  recv : process / suspectOrDeadNode' / aliveNode (Core.hs:89-121,142-218)
 //
 // Mapping to the hardware (integer / indexing work, no tensor cores by design):
-//   * K1a streams ONE 16-byte `meta` record per node (alive / suspect / crashed-member bitmaps +
-//     flags); a lane handles 8 nodes (8 independent 128-bit loads, two Philox4x32-10 calls — four
-//     nodes share a block —, eight r-th-set-bit picks); a warp covers 4 KB contiguous.
+//   * K1a streams ONE 4-byte summary word per node (up, piggyback count, min(L, 4), suspect, exposed); a lane handles 8
+//     nodes (2 independent 128-bit loads); only exposed nodes (a crashed process in an Alive slot) gather their 16-byte
+//     `meta` record (alive / suspect / crashed-member bitmaps) and spend Philox4x32-10 blocks — four nodes share a
+//     block — and r-th-set-bit picks; a warp covers 1 KB contiguous.
 //   * nodes that need more than the read-only probe (a countdown to run, a failed probe, a non-empty
 //     piggyback buffer) go to a work list (warp-aggregated append) and are handled warp-per-node:
 //     lane s owns view slot s, the piggyback buffer is staged in shared memory, membership lookups
@@ -98,8 +99,12 @@ struct SimDev {
   uint32_t *in_off;          // [n+1]
   uint32_t *in_src;          // [E] sender ids, ascending per receiver
   uint8_t *eflag;            // [E] 1 = sender mailed this round
-  uint4 *meta;               // [n*W] per 32 slots: {alive bitmap, suspect bitmap, crashed-member bitmap,
-                             //        flags: byte0 = process up, byte1 = piggyback count (word 0 only)}
+  uint4 *meta;               // [n*W] per 32 slots: {alive bitmap, suspect bitmap, crashed-member bitmap, unused}
+  // [n] per node, what the scan reads (a lane's Philox group of four nodes is one 16-byte load): byte 0 = process up,
+  // byte 1 = piggyback count, byte 2 = min(L, 4) (L = Alive slots; P <= SWIM_MAX_PROBES = 4) | some slot Suspect << 3 |
+  // exposed << 4. Exposed: a crashed process may sit in an Alive slot (am & td != 0). Every other field is exact; the
+  // exposed bit may be set spuriously (that costs the scan one meta gather) but is never clear for an exposed node.
+  uint32_t *nsum;
   uint32_t *obs_off;         // [N+1] observers of member m among this shard's rows ...
   uint32_t *obs_slot;        // [n*cap] ... as linear slot indices l*cap + s
   uint32_t *wl, *wl_cnt;     // work lists of K1b [2][n] (round parity); counters indexed by round % 3
@@ -413,13 +418,22 @@ __device__ __forceinline__ void pb_load(PbStage &p, const SimDev &d, uint32_t l,
   __syncwarp();
 }
 
-__device__ __forceinline__ void pb_store(PbStage &p, const SimDev &d, uint32_t l, int lane) {
+// Fields of the summary word SimDev::nsum.
+constexpr uint32_t kNsPb = 0xFF00u, kNsSus = 1u << 19, kNsExposed = 1u << 20;
+constexpr uint32_t kNsBusy = kNsPb | kNsSus; // the word alone sends a live node to K1b
+__device__ __forceinline__ uint32_t ns_up(uint32_t s) { return s & 0xFFu; }
+__device__ __forceinline__ uint32_t ns_alive(uint32_t s) { return s >> 16 & 7u; } // min(L, 4)
+
+// atomic_ns: the caller is event_kernel, where another warp's crash event may set the exposed bit of the same summary
+// word at the same time; there every update of the word is an atomic on all 32 bits.
+__device__ __forceinline__ void pb_store(PbStage &p, const SimDev &d, uint32_t l, int lane, bool atomic_ns = false) {
   if (!p.dirty) return;
   __syncwarp();
   if ((uint32_t)lane < p.cnt) d.pb[(size_t)l * d.B + lane] = p.s[lane];
   if (lane == 0) {
     d.pb_cnt[l] = (uint8_t)p.cnt;
-    reinterpret_cast<uint8_t *>(d.meta + (size_t)l * (d.cap >> 5))[13] = (uint8_t)p.cnt; // flags byte 1
+    if (atomic_ns) { atomicAnd(&d.nsum[l], ~kNsPb); atomicOr(&d.nsum[l], p.cnt << 8); }
+    else reinterpret_cast<uint8_t *>(d.nsum + l)[1] = (uint8_t)p.cnt;
   }
 }
 
@@ -465,8 +479,12 @@ __device__ __forceinline__ void row_load(Row<W> &r, const SimDev &d, uint32_t l,
   r.ticked = 0;
 }
 
+// td: the row's crashed-member bits, for the exposed bit of the summary word. In the round kernels they cannot change, so
+// the byte is stored exactly; in event_kernel (atomic_ns) a crash event of another warp may be setting them, so the
+// exposed bit is only ever set there (mark_observers sets it on every crash).
 template <int W>
-__device__ __forceinline__ void row_store(const Row<W> &r, const SimDev &d, uint32_t l, int lane, uint32_t round) {
+__device__ __forceinline__ void row_store(const Row<W> &r, const SimDev &d, uint32_t l, int lane, uint32_t round,
+                                          const uint32_t (&td)[W], bool atomic_ns = false) {
   size_t base = (size_t)l * d.cap + lane;
 #pragma unroll
   for (int w = 0; w < W; ++w) {
@@ -478,7 +496,8 @@ __device__ __forceinline__ void row_store(const Row<W> &r, const SimDev &d, uint
       d.vst[base + w * 32] = (uint8_t)r.st[w];
     }
   }
-  if (__any_sync(kFull, r.touched != 0)) { // liveness changed somewhere: refresh the row's bitmaps
+  if (__any_sync(kFull, r.touched != 0)) { // liveness changed somewhere: refresh the row's bitmaps and its summary byte
+    uint32_t acc = 0; // L in bits 0-8, some slot Suspect: bit 16, exposed: bit 17 (one register across the loop)
 #pragma unroll
     for (int w = 0; w < W; ++w) {
       const unsigned am = __ballot_sync(kFull, (r.st[w] & 3u) == SWIM_ALIVE);
@@ -487,7 +506,20 @@ __device__ __forceinline__ void row_store(const Row<W> &r, const SimDev &d, uint
         uint32_t *m = reinterpret_cast<uint32_t *>(d.meta + (size_t)l * W + w);
         m[0] = am;
         m[1] = sm;
+        if constexpr (W >= 8) { // wide rows: the crashed-member word is read back, which keeps td out of this loop's registers
+          acc += __popc(am);
+          acc |= (sm ? 1u << 16 : 0u) | ((am & m[2]) ? 1u << 17 : 0u);
+        }
       }
+      if constexpr (W < 8) {
+        acc += __popc(am);
+        acc |= (sm ? 1u << 16 : 0u) | ((am & td[w]) ? 1u << 17 : 0u);
+      }
+    }
+    if (lane == 0) {
+      const uint32_t L = acc & 0x1FFu, b2 = (L < 4u ? L : 4u) | (acc >> 16 & 1u) << 3 | (acc >> 17 & 1u) << 4;
+      if (atomic_ns) { atomicAnd(&d.nsum[l], ~(0xFu << 16)); atomicOr(&d.nsum[l], b2 << 16); }
+      else reinterpret_cast<uint8_t *>(d.nsum + l)[2] = (uint8_t)b2;
     }
   }
 }
@@ -699,14 +731,21 @@ __device__ __forceinline__ bool probe_fails(const SimDev &d, uint32_t (&am)[W], 
   }
   return fails;
 }
+// probe_fails of a node that is not exposed (am & td == 0): every pick lands on a live target, in random and round-robin
+// order alike, so the period fails iff the direct leg of one of its nt = min(P, L) probes is lost. Needs no bitmaps.
+__device__ __forceinline__ bool probe_lost(const SimDev &d, uint32_t nt, uint32_t ldraw, uint32_t round, uint32_t self) {
+  bool lost = bounded(ldraw, 1000000u) < d.loss_ppm;
+  for (uint32_t j = 1; j < nt; ++j) lost |= direct_leg_lost(d, round, self, j);
+  return lost;
+}
 
 // A node's tick decision — does it need K1b in this round? A crashed process does nothing. A buffered record to send or
 // a countdown to run [Q8] means work. Otherwise only a failed probe can, and only if a crashed process sits in an Alive
 // slot or messages can be lost: then the probe decides (probe_fails, on the node's draws). Without either, whichever slot
 // a draw selects, the Ack comes back, so the picks and the Philox blocks behind them are not needed — the common case.
-// The rule is stated from a node's meta words by node_needs_work (the wide-row scan, the batched quiet scan and, with the
-// draws made early, the receive pass) and from a view row a warp has loaded by tick_decide and x_node; the W == 1 scan
-// restates it inline. Each form is written for the register budget of the kernels it sits in: one shared row form, used by
+// The rule is stated from a node's summary word by the scans (scan_pass, quiet_scan: bitmaps only for exposed nodes), from
+// bitmaps by node_needs_work (the receive pass, with the draws made early) and from a view row a warp has loaded by
+// tick_decide and x_node. Each form is written for the register budget of the kernels it sits in: one shared row form, used by
 // recv_one and x_node too, made ptxas spill more in several round-kernel instances (DESIGN.md §5).
 
 // From the meta words; counts the node's Pings as well.
@@ -756,51 +795,51 @@ __device__ __forceinline__ void tick_decide(const SimDev &d, uint32_t tick_round
   }
 }
 
-// The meta records (word 0) of the 4 U nodes a lane takes in one trip of a scan: m[u][j] = node 4 (gb + 32 u + lane) + j.
-// Returns the nodes that lie in the shard (bit 4 u + j).
-template <int W>
-__device__ __forceinline__ uint32_t load_meta_group(const SimDev &d, uint32_t gb, int lane, uint4 (&m)[kScanGroups][4]) {
+// The summary words of the 4 U nodes a lane takes in one trip of a scan: word j of s[u] = node 4 (gb + 32 u + lane) + j
+// (0 outside the shard). Returns the nodes that lie in the shard (bit 4 u + j).
+__device__ __forceinline__ uint32_t load_nsum_group(const SimDev &d, uint32_t gb, int lane, uint4 (&s)[kScanGroups]) {
   constexpr int U = kScanGroups;
   uint32_t valid = 0;
-  if (4 * gb >= d.first && 4 * (gb + 32 * U) <= d.first + d.n) { // an interior warp: all 128 U nodes are the shard's
-    const uint4 *p = d.meta + (size_t)(4 * (gb + lane) - d.first) * W;
+  if ((d.first & 3u) == 0 && 4 * gb >= d.first && 4 * (gb + 32 * U) <= d.first + d.n) { // an interior warp: all its nodes are the shard's
+    const uint4 *p = reinterpret_cast<const uint4 *>(d.nsum + 4 * (gb + lane) - d.first);
 #pragma unroll
-    for (int u = 0; u < U; ++u)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) m[u][j] = p[(size_t)(u * 128 + j) * W]; // 4*U independent 16-byte loads in flight
+    for (int u = 0; u < U; ++u) s[u] = p[u * 32]; // U independent 16-byte loads in flight, 512 contiguous bytes per warp each
     valid = (1u << (4 * U)) - 1u;
   } else {
 #pragma unroll
-    for (int u = 0; u < U; ++u)
+    for (int u = 0; u < U; ++u) {
+      uint32_t w[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const uint32_t node = 4 * (gb + u * 32 + lane) + j;
         const bool ok = node >= d.first && node < d.first + d.n;
         valid |= (uint32_t)ok << (u * 4 + j);
-        m[u][j] = ok ? d.meta[(size_t)(node - d.first) * W] : make_uint4(0, 0, 0, 0);
+        w[j] = ok ? d.nsum[node - d.first] : 0u;
       }
+      s[u] = make_uint4(w[0], w[1], w[2], w[3]);
+    }
   }
   return valid;
 }
 
-// Local node l's bitmaps from its meta words: word 0 (m0) is already loaded, words 1 .. W-1 are loaded here.
+// Local node l's alive and crashed-member bitmaps (an exposed node's: the scans need them for no other).
 template <int W>
-__device__ __forceinline__ void node_meta(const SimDev &d, uint32_t l, uint4 m0, uint32_t (&am)[W], uint32_t (&td)[W], uint32_t &sus) {
-  am[0] = m0.x; td[0] = m0.z; sus = m0.y;
+__device__ __forceinline__ uint32_t node_meta(const SimDev &d, uint32_t l, uint32_t (&am)[W], uint32_t (&td)[W]) {
+  uint32_t L = 0;
 #pragma unroll
-  for (int w = 1; w < W; ++w) {
+  for (int w = 0; w < W; ++w) {
     const uint4 mw = d.meta[(size_t)l * W + w];
-    am[w] = mw.x; sus |= mw.y; td[w] = mw.z;
+    am[w] = mw.x; td[w] = mw.z;
+    L += __popc(mw.x);
   }
+  return L;
 }
 
-// K1a — streaming pass over every node of the shard, EIGHT nodes per lane: the four nodes 4g..4g+3
-// share one Philox4x32-10 block (one 32-bit draw each), so a lane issues eight independent 16-byte
-// loads (the nodes' meta records: alive / suspect / crashed-member bitmaps + flags), two Philox
-// calls, and eight r-th-set-bit picks (shuffle, Util.hs:36-42) tested against the crashed-member
-// bitmap. A warp covers 256 consecutive nodes = 4 KB contiguous. Nodes that need more — a Suspect
-// slot to count down, a failed probe, a non-empty piggyback buffer — are appended to the round's
-// work list for K1b.
+// K1a — streaming pass over every node of the shard, EIGHT nodes per lane: a lane loads the summary words (SimDev::nsum)
+// of two Philox groups of four nodes, two 16-byte loads; a warp covers 256 consecutive nodes = 1 KB contiguous. Only an
+// exposed node gathers its meta bitmaps and spends a Philox block (four nodes share one) and r-th-set-bit picks (shuffle,
+// Util.hs:36-42) tested against the crashed-member bitmap. Nodes that need more — a Suspect slot to count down, a failed
+// probe, a non-empty piggyback buffer — are appended to the round's work list for K1b.
 template <int W>
 __device__ __forceinline__ void scan_pass(const SimDev &d, uint32_t round, uint32_t warp, uint32_t nwarps,
                                           int lane, uint32_t &pings, const uint32_t *skipbits = nullptr,
@@ -812,19 +851,8 @@ __device__ __forceinline__ void scan_pass(const SimDev &d, uint32_t round, uint3
   uint32_t *const wl = wl_of(d, round);
   const uint32_t g0 = d.first >> 2, g1 = (d.first + d.n + 3) >> 2; // Philox groups touching this shard
   for (uint32_t gb = g0 + warp * (32 * U); gb < g1; gb += nwarps * (32 * U)) {
-    uint4 m[U][4];
-    uint32_t valid = load_meta_group<W>(d, gb, lane, m); // bit u*4+j
-    uint32_t up = 0, busy = 0; // W == 1, bit u*4+j: the node's process is up / its record alone sends it to K1b
-    if constexpr (W == 1) {
-      // of a record, pass 1 below needs x, z and these two bits: folded right away, the eight records take 16 registers
-      // instead of 32 for the rest of the trip
-#pragma unroll
-      for (int q = 0; q < 4 * U; ++q) {
-        const uint4 mr = m[q >> 2][q & 3];
-        up |= (uint32_t)((mr.w & 0xFFu) != 0) << q;
-        busy |= (uint32_t)((mr.w & 0xFF00u) != 0 || mr.y != 0) << q;
-      }
-    }
+    uint4 s[U];
+    uint32_t valid = load_nsum_group(d, gb, lane, s); // bit u*4+j
     if ((skipbits || skipbits2) && valid == (1u << (4 * U)) - 1u && (d.first & 3u) == 0) {
       // (the lane's four nodes of a group are consecutive and 4-aligned in the shard: one bitmap word holds their bits)
 #pragma unroll
@@ -851,93 +879,85 @@ __device__ __forceinline__ void scan_pass(const SimDev &d, uint32_t round, uint3
     uint32_t work = 0; // bit u*4+j: that node needs K1b
     unsigned fb = 0;     // lanes whose STAGED node (see below) needs K1b ...
     uint32_t fself = 0;  // ... and that node's id
-    if constexpr (W == 1) {
-      // Pass 1, every node: what the record alone decides (buffer to send, countdown to run, the Ping count). Only a node
-      // with a crashed process in an Alive slot (or any node, under message loss) depends on its draws — and only if the
-      // record has not already sent it to K1b. Those nodes are COMPACTED over the warp through `stage` (32 entries of the
-      // warp's shared memory: {alive bitmap, crashed-member bitmap, id}): pass 2 then spends one Philox block and one set
-      // of picks per lane on up to 32 of them at once, whichever lanes they came from (a burst round of C3 has ~8 per
-      // warp: one trip instead of the two or three a per-lane loop needs). Without a stage buffer, under message loss
-      // (every node is risky) and for the overflow, the per-lane loop below does the same work.
-      uint32_t risky = 0, nstaged = 0;
-      const bool can_stage = stage != nullptr && d.loss_ppm == 0;
+    // Pass 1, every node: what the summary word alone decides (buffer to send, countdown to run, the Ping count). Only an
+    // exposed node (or any node, under message loss) depends on its draws — and only if the word has not already sent it
+    // to K1b. Those nodes are COMPACTED over the warp through `stage` (the ids of up to 32, in the warp's shared memory):
+    // the staged pass then spends one meta gather, one Philox block and one set of picks per lane on up to 32 of them at
+    // once, whichever lanes they came from (a burst round of C3 has ~8 per warp: one trip instead of the two or three a
+    // per-lane loop needs). Without a stage buffer, under message loss (every node is risky) and for the overflow, the
+    // per-lane loop below does the same work.
+    uint32_t risky = 0, nstaged = 0;
+    const bool can_stage = stage != nullptr && d.loss_ppm == 0;
+    uint32_t *const sid = reinterpret_cast<uint32_t *>(stage);
 #pragma unroll
-      for (int u = 0; u < U; ++u)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int q = u * 4 + j;
-          const uint4 mr = m[u][j];
-          bool rq = false;
-          if (valid >> q & up >> q & 1u) { // in range, not left to the receive pass, process up
-            const uint32_t L = __popc(mr.x);
-            const bool wk = busy >> q & 1u;
-            if (wk) work |= 1u << q;
-            if (L) {
-              pings += d.P < L ? d.P : L;
-              rq = !wk && ((mr.x & mr.z) | d.loss_ppm) != 0;
-            }
-          }
-          if (can_stage) {
-            const unsigned rb = __ballot_sync(kFull, rq);
-            if (rb) {
-              const uint32_t pos = nstaged + __popc(rb & ((1u << lane) - 1u));
-              if (rq) {
-                if (pos < 32u) stage[pos] = make_uint4(mr.x, mr.z, 4 * (gb + u * 32 + lane) + j, 0u);
-                else risky |= 1u << q; // (more than 32 in one warp's 256 nodes: the per-lane loop takes the rest)
-              }
-              nstaged += __popc(rb);
-            }
-          } else if (rq) {
-            risky |= 1u << q;
-          }
-        }
-      // Pass 2 takes the nodes that were not staged one per lane and trip (Philox block, r-th-set-bit picks): a lane pays
-      // for its own risky nodes only, not — by divergence — for every risky node of the warp. It runs ahead of the staged
-      // picks, which need none of the records: the records are dead by then, and the staged pass keeps its registers.
-      while (risky) {
-        const int q = __ffs(risky) - 1;
-        risky &= risky - 1;
-        uint32_t am1[1] = {0}, td1[1] = {0};
-#pragma unroll
-        for (int qq = 0; qq < 4 * U; ++qq)
-          if (q == qq) { am1[0] = m[qq >> 2][qq & 3].x; td1[0] = m[qq >> 2][qq & 3].z; }
-        const uint32_t g = gb + (q >> 2) * 32 + lane, self = 4 * g + (q & 3);
-        const uint4 x = target_block<W>(d, round, g);
-        uint32_t ldraw = 0;
-        if (d.loss_ppm) ldraw = word_of(philox4x32_10(make_uint4(round, g, P_LOSS0, 0), d.key0, d.key1), q & 3);
-        if (probe_fails<W>(d, am1, td1, (uint32_t)__popc(am1[0]), word_of(x, q & 3), ldraw, round, self)) work |= 1u << q;
-      }
-      // ... and the staged nodes, up to 32 at once
-      if (nstaged) {
-        __syncwarp();
-        bool fails = false;
-        if ((uint32_t)lane < (nstaged < 32u ? nstaged : 32u)) {
-          const uint4 e = stage[lane];
-          uint32_t am1[1] = {e.x}, td1[1] = {e.y};
-          const uint4 x = target_block<W>(d, round, e.z >> 2);
-          fails = probe_fails<W>(d, am1, td1, (uint32_t)__popc(e.x), word_of(x, e.z & 3), 0u, round, e.z);
-          fself = e.z;
-        }
-        fb = __ballot_sync(kFull, fails);
-        __syncwarp(); // the buffer is free again (next trip of this loop, or the passes that follow the scan)
-      }
-    } else {
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const uint32_t g = gb + u * 32 + lane;
-      if ((valid >> (u * 4) & 0xFu) == 0) continue;
-      uint4 x = target_block<W>(d, round, g);
-      uint4 y = make_uint4(0, 0, 0, 0);
-      if (d.loss_ppm) y = philox4x32_10(make_uint4(round, g, P_LOSS0, 0), d.key0, d.key1);
+    for (int u = 0; u < U; ++u)
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        if (!(valid >> (u * 4 + j) & 1u)) continue;
-        uint32_t am[W], td[W], sus;
-        node_meta<W>(d, 4 * g + j - d.first, m[u][j], am, td, sus);
-        const bool need = node_needs_work<W>(d, m[u][j].w, am, td, sus, word_of(x, j), word_of(y, j), round, pings, 4 * g + j);
-        work |= (uint32_t)need << (u * 4 + j);
+        const int q = u * 4 + j;
+        const uint32_t sw = word_of(s[u], j);
+        bool rq = false;
+        if ((valid >> q & 1u) && ns_up(sw)) { // in range, not left to the receive pass, process up
+          const uint32_t L = ns_alive(sw);
+          const bool wk = (sw & kNsBusy) != 0;
+          if (wk) work |= 1u << q;
+          if (L) {
+            pings += d.P < L ? d.P : L;
+            rq = !wk && ((sw & kNsExposed) || d.loss_ppm);
+          }
+        }
+        if (can_stage) {
+          const unsigned rb = __ballot_sync(kFull, rq);
+          if (rb) {
+            const uint32_t pos = nstaged + __popc(rb & ((1u << lane) - 1u));
+            if (rq) {
+              if (pos < 32u) sid[pos] = 4 * (gb + u * 32 + lane) + j;
+              else risky |= 1u << q; // (more than 32 in one warp's 256 nodes: the per-lane loop takes the rest)
+            }
+            nstaged += __popc(rb);
+          }
+        } else if (rq) {
+          risky |= 1u << q;
+        }
       }
+    // The nodes that were not staged, one per lane and trip: a lane pays for its own risky nodes only, not — by
+    // divergence — for every risky node of the warp. An exposed node gathers its bitmaps and runs the picks; any other
+    // only asks whether a direct leg is lost (probe_lost).
+    while (risky) {
+      const int q = __ffs(risky) - 1;
+      risky &= risky - 1;
+      uint32_t sw = 0;
+#pragma unroll
+      for (int qq = 0; qq < 4 * U; ++qq)
+        if (q == qq) sw = word_of(s[qq >> 2], qq & 3);
+      const uint32_t g = gb + (q >> 2) * 32 + lane, self = 4 * g + (q & 3);
+      uint32_t ldraw = 0;
+      if (d.loss_ppm) ldraw = word_of(philox4x32_10(make_uint4(round, g, P_LOSS0, 0), d.key0, d.key1), q & 3);
+      bool fails;
+      if (sw & kNsExposed) {
+        uint32_t am[W], td[W];
+        const uint32_t L = node_meta<W>(d, self - d.first, am, td);
+        const uint4 x = target_block<W>(d, round, g);
+        fails = probe_fails<W>(d, am, td, L, word_of(x, q & 3), ldraw, round, self);
+      } else {
+        const uint32_t L = ns_alive(sw);
+        fails = probe_lost(d, d.P < L ? d.P : L, ldraw, round, self);
+      }
+      if (fails) work |= 1u << q;
     }
+    // ... and the staged nodes (all exposed: staging is off under message loss), up to 32 at once
+    if (nstaged) {
+      __syncwarp();
+      bool fails = false;
+      if ((uint32_t)lane < (nstaged < 32u ? nstaged : 32u)) {
+        const uint32_t self = sid[lane];
+        uint32_t am[W], td[W];
+        const uint32_t L = node_meta<W>(d, self - d.first, am, td); // (in flight while the Philox block is computed)
+        const uint4 x = target_block<W>(d, round, self >> 2);
+        fails = probe_fails<W>(d, am, td, L, word_of(x, self & 3), 0u, round, self);
+        fself = self;
+      }
+      fb = __ballot_sync(kFull, fails);
+      __syncwarp(); // the buffer is free again (next trip of this loop, or the passes that follow the scan)
     }
     // warp-aggregated append of up to 4*U x 32 nodes
     if (__any_sync(kFull, work != 0) || fb) {
@@ -981,9 +1001,9 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) tick_scan_kernel(SimDev 
 }
 
 // K1a over Q consecutive rounds at once, for stretches in which nothing happens. A round whose scan lists no work
-// writes nothing, so the scan of the round after it reads the same meta records: one pass loads them once and decides
+// writes nothing, so the scan of the round after it reads the same summary words: one pass loads them once and decides
 // rounds round .. round+Q-1 together. Only the probe outcome depends on the round (through the target draw), and only
-// for nodes that have a crashed process in an Alive slot — rare once a cluster has converged; everything else a node
+// for exposed nodes (a crashed process in an Alive slot) — rare once a cluster has converged; everything else a node
 // can need (a buffered record, a countdown) holds for every round of the batch. Nothing is listed: the result is the
 // lane's mask of rounds that are NOT quiet (bit q: round + q), the caller commits the rounds before the first such bit
 // and runs the ordinary scan from there. `pings` is the Ping count of ONE round (the same for each of them).
@@ -996,32 +1016,28 @@ __device__ __forceinline__ uint32_t quiet_scan(const SimDev &d, uint32_t round, 
   uint32_t busy = 0;
   const uint32_t g0 = d.first >> 2, g1 = (d.first + d.n + 3) >> 2;
   for (uint32_t gb = g0 + warp * (32 * U); gb < g1; gb += nwarps * (32 * U)) {
-    uint4 m[U][4];
-    const uint32_t valid = load_meta_group<W>(d, gb, lane, m);
+    uint4 s[U];
+    const uint32_t valid = load_nsum_group(d, gb, lane, s);
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       const uint32_t g = gb + u * 32 + lane;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        if (!(valid >> (u * 4 + j) & 1u)) continue;
-        uint32_t am[W], td[W], sus, risk = 0;
-        node_meta<W>(d, 4 * g + j - d.first, m[u][j], am, td, sus);
-#pragma unroll
-        for (int w = 0; w < W; ++w) risk |= am[w] & td[w];
-        if (!risk) { // the draw is never looked at: one decision for the whole batch
-          if (node_needs_work<W>(d, m[u][j].w, am, td, sus, 0, 0, round, pings, 4 * g + j)) busy = allq;
-          continue;
-        }
-        uint32_t p = 0;
+        const uint32_t sw = word_of(s[u], j), L = ns_alive(sw);
+        if (!(valid >> (u * 4 + j) & 1u) || !ns_up(sw)) continue;
+        if (sw & kNsBusy) busy = allq;
+        if (!L) continue;
+        pings += d.P < L ? d.P : L;
+        if ((sw & kNsBusy) || !(sw & kNsExposed)) continue; // the draw is never looked at: one decision for the batch
+        uint32_t am[W], td[W];
+        const uint32_t Lt = node_meta<W>(d, 4 * g + j - d.first, am, td);
         for (uint32_t q = 0; q < Q; ++q) {
           uint32_t amq[W];
 #pragma unroll
           for (int w = 0; w < W; ++w) amq[w] = am[w];
           const uint4 x = target_block<W>(d, round + q, g);
-          p = 0;
-          if (node_needs_work<W>(d, m[u][j].w, amq, td, sus, word_of(x, j), 0, round + q, p, 4 * g + j)) busy |= 1u << q;
+          if (probe_fails<W>(d, amq, td, Lt, word_of(x, j), 0, round + q, 4 * g + j)) busy |= 1u << q;
         }
-        pings += p;
       }
     }
   }
@@ -1161,7 +1177,7 @@ __device__ __forceinline__ void work_body(const SimDev &d, uint32_t round, uint3
       }
     }
   }
-  row_store<W>(row, d, ln, lane, round);
+  row_store<W>(row, d, ln, lane, round, td);
 #ifndef SWIM_EMU
   if (have_next && lane < 5) { // next item's rows -> L2 (one 128-byte line each at cap 32)
     const size_t nb = (size_t)next_ln * d.cap;
@@ -1456,7 +1472,10 @@ __device__ __forceinline__ void recv_one(const SimDev &d, uint32_t round, uint32
   if (__shfl_sync(kFull, old, 0) == round) return; // another warp has this receiver
   // (a listed receiver is a live process: senders deliver only to members whose crashed-member bit is clear)
   apply_mail<W>(d, round, ln, e0, e1, early, snd, early_rec, early_cnt, row, pbs, self_inc, lane, c);
-  row_store<W>(row, d, ln, lane, round);
+  if (!tick_round) // row_store needs them too (loaded only now: not held across the mail without a tick decision)
+#pragma unroll
+    for (int w = 0; w < W; ++w) td[w] = d.meta[(size_t)ln * W + w].z;
+  row_store<W>(row, d, ln, lane, round, td);
   pb_store(pbs, d, ln, lane);
   if (lane == 0 && self_inc != self_inc0) d.self_inc[ln] = self_inc;
   if (tick_round) {
@@ -1824,7 +1843,7 @@ __device__ __forceinline__ void x_node(const SimDev &d, uint32_t round, uint32_t
     for (int w = 0; w < W; ++w) l_pre += __popc(__ballot_sync(kFull, (row.st[w] & 3u) == SWIM_ALIVE));
     const uint32_t self_inc0 = self_inc;
     apply_mail<W>(d, mround, ln, e0, e1, early, snd, early_rec, early_cnt, row, pbs, self_inc, lane, c);
-    row_store<W>(row, d, ln, lane, mround); // (lastChange = the round of the mail)
+    row_store<W>(row, d, ln, lane, mround, td); // (lastChange = the round of the mail)
     row.touched = 0;
     row.ticked = 0;
     if (lane == 0 && self_inc != self_inc0) d.self_inc[ln] = self_inc;
@@ -1984,34 +2003,44 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) round_kernel_x(SimDev d)
 
 // =================================================================== events (phase E)
 // Keep the crashed-member bitmaps in step with alive[]: every row of this shard that lists
-// `node` has the corresponding bit set (crash) or cleared (rejoin).
+// `node` has the corresponding bit set (crash) or cleared (rejoin), and a crash marks the row exposed.
 __device__ __forceinline__ void mark_observers(const SimDev &d, uint32_t node, bool crashed, int lane) {
   const uint32_t W = d.cap >> 5;
   for (uint32_t x = d.obs_off[node] + lane, end = d.obs_off[node + 1]; x < end; x += 32) {
     const uint32_t slot = d.obs_slot[x], l = slot / d.cap, s = slot % d.cap;
     uint32_t *word = reinterpret_cast<uint32_t *>(d.meta + (size_t)l * W + (s >> 5)) + 2;
-    if (crashed) atomicOr(word, 1u << (s & 31)); else atomicAnd(word, ~(1u << (s & 31)));
+    if (crashed) {
+      atomicOr(word, 1u << (s & 31));
+      atomicOr(&d.nsum[l], kNsExposed); // whatever the slot's liveness: an INJECT on row l may be making it Alive right now
+    } else {
+      atomicAnd(word, ~(1u << (s & 31))); // (the exposed bit stays: spurious until the row's next store, never missing)
+    }
   }
 }
 
-// Rebuild every per-node meta record from the primary arrays (after bulk edits of alive[], rows
+// Rebuild every per-node meta record and summary word from the primary arrays (after bulk edits of alive[], rows
 // or buffers through the ABI): bitmaps from the row's liveness, crashed members from alive[nbr].
 static __global__ void __launch_bounds__(kThreads) derive_meta_kernel(SimDev d) {
   const int lane = threadIdx.x & 31;
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
   const uint32_t W = d.cap >> 5;
-  for (uint32_t l = warp; l < d.n; l += nwarps)
+  for (uint32_t l = warp; l < d.n; l += nwarps) {
+    uint32_t L = 0, sus = 0, ex = 0;
     for (uint32_t w = 0; w < W; ++w) {
       const size_t x = (size_t)l * d.cap + w * 32 + lane;
       const uint32_t live = d.vst[x] & 3u;
       const unsigned am = __ballot_sync(kFull, live == SWIM_ALIVE);
       const unsigned sm = __ballot_sync(kFull, live == SWIM_SUSPECT);
       const unsigned td = __ballot_sync(kFull, live != SWIM_VACANT && d.alive[d.nbr[x]] == 0);
-      if (lane == 0) {
-        const uint32_t flags = w == 0 ? (d.alive[d.first + l] ? 1u : 0u) | ((uint32_t)d.pb_cnt[l] << 8) : 0u;
-        d.meta[(size_t)l * W + w] = make_uint4(am, sm, td, flags);
-      }
+      if (lane == 0) d.meta[(size_t)l * W + w] = make_uint4(am, sm, td, 0u);
+      L += __popc(am);
+      sus |= sm;
+      ex |= am & td;
     }
+    if (lane == 0)
+      d.nsum[l] = (d.alive[d.first + l] ? 1u : 0u) | ((uint32_t)d.pb_cnt[l] << 8) |
+                  ((L < 4u ? L : 4u) << 16) | (sus ? kNsSus : 0u) | (ex ? kNsExposed : 0u);
+  }
 }
 
 struct DevEvent {
@@ -2090,7 +2119,7 @@ __global__ void __launch_bounds__(kThreads) event_kernel(SimDev d, const DevEven
       if (lane == 0) {
         d.alive[node] = 0;
         if (was_up) d.last_crash[node] = round;
-        if (local) reinterpret_cast<uint8_t *>(d.meta + (size_t)ln * (d.cap >> 5))[12] = 0; // flags byte 0: up
+        if (local) atomicAnd(&d.nsum[ln], ~0xFFu); // byte 0: up
       }
       mark_observers(d, node, true, lane);
     } else if (kind == SWIM_EV_REJOIN) {
@@ -2100,7 +2129,7 @@ __global__ void __launch_bounds__(kThreads) event_kernel(SimDev d, const DevEven
         if (lane == 0) {
           d.alive[node] = 1;
           d.last_rejoin[node] = round;
-          if (local) reinterpret_cast<uint8_t *>(d.meta + (size_t)ln * (d.cap >> 5))[12] = 1;
+          if (local) atomicOr(&d.nsum[ln], 1u);
         }
         mark_observers(d, node, false, lane);
         if (local) { // restart with incarnation + 1 and announce Alive
@@ -2109,13 +2138,16 @@ __global__ void __launch_bounds__(kThreads) event_kernel(SimDev d, const DevEven
           if (lane == 0) d.self_inc[ln] = inc;
           pb_load(pbs, d, ln, lane);
           pb_enqueue(pbs, d, make_rec(node, inc, 0, SWIM_MSG_ALIVE), lane, c.v[SWIM_CTR_PB_DROPPED]);
-          pb_store(pbs, d, ln, lane);
+          pb_store(pbs, d, ln, lane, true);
         }
       }
     } else if (local && d.alive[node] != 0) { // SWIM_EV_INJECT: one datagram through `process`
       Row<W> row;
       row_load<W>(row, d, ln, lane);
       pb_load(pbs, d, ln, lane);
+      uint32_t td[W];
+#pragma unroll
+      for (int w = 0; w < W; ++w) td[w] = d.meta[(size_t)ln * W + w].z;
       uint32_t self_inc = d.self_inc[ln];
       const uint32_t self_inc0 = self_inc;
       uint4 rb;
@@ -2123,8 +2155,8 @@ __global__ void __launch_bounds__(kThreads) event_kernel(SimDev d, const DevEven
         pb_enqueue(pbs, d, rb, lane, c.v[SWIM_CTR_PB_DROPPED]);
         if (lane == 0) ++c.v[SWIM_CTR_RECS_APPLIED];
       }
-      row_store<W>(row, d, ln, lane, round);
-      pb_store(pbs, d, ln, lane);
+      row_store<W>(row, d, ln, lane, round, td, true);
+      pb_store(pbs, d, ln, lane, true);
       if (lane == 0 && self_inc != self_inc0) d.self_inc[ln] = self_inc;
     }
     __syncwarp();
@@ -2180,10 +2212,9 @@ __device__ __forceinline__ uint32_t count_mismatches(const SimDev &d) {
   const uint32_t W = d.cap >> 5;
   uint32_t bad = 0;
   for (size_t l = (size_t)blockIdx.x * blockDim.x + threadIdx.x; l < d.n; l += (size_t)gridDim.x * blockDim.x) {
-    const uint4 m0 = d.meta[l * W];
-    if ((m0.w & 0xFFu) == 0) continue; // a crashed observer's view does not count
+    if (!ns_up(d.nsum[l])) continue; // a crashed observer's view does not count
     for (uint32_t w = 0; w < W; ++w) {
-      const uint4 m = w ? d.meta[l * W + w] : m0;
+      const uint4 m = d.meta[l * W + w];
       bad += __popc(m.z & (m.x | m.y)) + __popc(m.y & ~m.z);
       uint32_t rest = ~(m.x | m.y | m.z);
       while (rest) {

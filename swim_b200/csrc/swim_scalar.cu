@@ -54,11 +54,13 @@ __global__ void scalar_kernel(SimDev d, ScalarArgs *a) {
     case OP_APPLY: { // suspectNode / deadNode / aliveNode (Core.hs:189-218)
       Row<W> row;
       row_load<W>(row, d, ln, lane);
+      uint32_t td[W];
+      for (int w = 0; w < W; ++w) td[w] = d.meta[(size_t)ln * W + w].z;
       uint32_t self_inc = d.self_inc[ln];
       const uint32_t self_inc0 = self_inc;
       uint4 rb = make_uint4(0, 0, 0, 0);
       int v = row_apply<W>(row, d, a->node, self_inc, a->rec, rb, lane, dummy);
-      row_store<W>(row, d, ln, lane, d.round);
+      row_store<W>(row, d, ln, lane, d.round, td);
       __syncwarp();
       if (lane == 0) {
         if (self_inc != self_inc0) d.self_inc[ln] = self_inc;
@@ -122,6 +124,8 @@ __global__ void scalar_kernel(SimDev d, ScalarArgs *a) {
     case OP_TICK_TIMERS: { // phase T1 for one store: the same countdown / expiry code as work_pass
       Row<W> row;
       row_load<W>(row, d, ln, lane);
+      uint32_t td[W];
+      for (int w = 0; w < W; ++w) td[w] = d.meta[(size_t)ln * W + w].z;
       PbStage pbs;
       pbs.s = s_pb;
       pb_load(pbs, d, ln, lane);
@@ -139,7 +143,7 @@ __global__ void scalar_kernel(SimDev d, ScalarArgs *a) {
           ++expired;
         }
       }
-      row_store<W>(row, d, ln, lane, d.round);
+      row_store<W>(row, d, ln, lane, d.round, td);
       pb_store(pbs, d, ln, lane);
       if (lane == 0) a->value = expired;
       break;

@@ -225,6 +225,7 @@ extern "C" int swim_sim_create(const swim_config_t *cfg, swim_sim_t **out) {
     if ((r = dalloc(sim, &d.ridx, slots, 0))) return r;
     if ((r = dalloc(sim, &d.in_off, n + 1, 0))) return r;
     if ((r = dalloc(sim, &d.meta, slots / 32, 0))) return r;
+    if ((r = dalloc(sim, &d.nsum, n, 0))) return r;
     if ((r = dalloc(sim, &d.obs_off, (size_t)d.N + 1, 0))) return r;
     if ((r = dalloc(sim, &d.obs_slot, slots, 0))) return r;
     if ((r = dalloc(sim, &d.wl, 2 * n, 0))) return r; // [parity]
@@ -682,7 +683,7 @@ static void ckpt_sources(const swim_sim *sim, std::vector<std::pair<void *, size
   v = {{d.alive, (size_t)d.N}, {d.back_at, (size_t)d.N * 4}, {d.last_crash, (size_t)d.N * 4}, {d.last_rejoin, (size_t)d.N * 4},
        {d.self_inc, n * 4}, {d.seqno, n * 4}, {d.vst, slots}, {d.vinc, slots * 4},
        {d.vlast, slots * 4}, {d.pb, n * d.B * sizeof(uint4)}, {d.pb_cnt, n}, {d.meta, slots / 32 * sizeof(uint4)},
-       {sim->d_scratch, (2 + SWIM_CTR__COUNT) * sizeof(unsigned long long)}};
+       {d.nsum, n * 4}, {sim->d_scratch, (2 + SWIM_CTR__COUNT) * sizeof(unsigned long long)}};
 }
 
 extern "C" int swim_sim_save(swim_sim_t *sim) {
