@@ -324,6 +324,20 @@ typedef struct swim_member_add {
 } swim_member_add_t;
 int swim_sim_add_members(swim_sim_t *sim, const swim_member_add_t *adds, size_t n, uint64_t *n_added, uint64_t *n_full);
 
+/* Push-pull state exchange between steps (DESIGN.md §2.6): memberlist's anti-entropy, the missing half of the
+ * reference's join (Config.joinHosts, Types.hs:47, is parsed and never used); the exchange itself has no reference
+ * counterpart. At the current round r (the round counter does not advance) every up node with at least one Alive slot
+ * picks one Alive member from the Philox block (r, node, 10, 0); if that partner is up, the two swap their full states
+ * (Alive(self), then every occupied slot as Alive / Suspect / Dead(from = sender)), read from a snapshot taken before
+ * anything changes. A receiver merges its senders in ascending id, each record through the receive rules; an Alive record
+ * about a member it does not list is inserted as swim_alive_node inserts (aliveNode / addNewMember, Core.hs:206-216), and
+ * dropped when the row is full. Two calls at the same round pick the same partners. No message is lost. Single shard
+ * only; SWIM_ESTATE when world > 1, before a view is installed and on a failed handle. Without inserts only state
+ * changes and the checkpoint stays valid; with inserts the view is marked changed as by the bulk edits above.
+ * Outputs may be NULL: *n_exchanges = choices whose partner was up, *n_inserted = members inserted, *n_full = inserts
+ * dropped on a full row. */
+int swim_sim_push_pull(swim_sim_t *sim, uint64_t *n_exchanges, uint64_t *n_inserted, uint64_t *n_full);
+
 /* Bulk copies of one state array (SWIM_ARR_*) between device and a host buffer of exactly
  * `bytes` bytes. set_array(SWIM_ARR_NBR) is rejected: use swim_sim_set_view. */
 int swim_sim_get_array(swim_sim_t *sim, int arr, void *host_buf, size_t bytes);

@@ -36,6 +36,8 @@ def main():
     ap.add_argument("--flags", type=int, default=0, help="SWIM_F_* protocol variants")
     ap.add_argument("--topology", default="random", choices=["random", "ring"])
     ap.add_argument("--sample-every", type=int, default=10)
+    ap.add_argument("--push-pull-every", type=int, default=0, metavar="R",
+                    help="a push-pull state exchange (memberlist anti-entropy) after every R-th round; one GPU only")
     ap.add_argument("--seed", type=int, default=0x5EED0001 + 5)
     args = ap.parse_args()
 
@@ -45,6 +47,9 @@ def main():
     from swim_b200.study import run_sweep_point
 
     rank, world, local = sd.init_from_env()
+    if args.push_pull_every and world > 1:
+        raise SystemExit("--push-pull-every needs one GPU: the exchange reads partners' rows, which live on other ranks "
+                         "when the simulation is sharded")
     if not torch.cuda.is_available():
         raise SystemExit("c5_suspicion_sweep needs a CUDA device (there is no CPU fallback)")
     torch.cuda.set_device(local)
@@ -77,7 +82,7 @@ def main():
         sim.set_params(suspicion_rounds=S, suspicion_max=min(smax, 15))
         barrier()
         t0 = time.perf_counter()
-        res = run_sweep_point(sim, None, args.rounds, args.sample_every, red)
+        res = run_sweep_point(sim, None, args.rounds, args.sample_every, red, args.push_pull_every)
         wall = time.perf_counter() - t0
         if rank == 0:
             rep = res["report"]
@@ -93,6 +98,9 @@ def main():
                     "node_rounds_per_s_device_rank0": n * args.rounds / max(1e-9, res["device_ms"] * 1e-3),
                     "node_rounds_per_s_wall": n * args.rounds / wall,
                     "setup_s": {"topology": t_topo, "create_set_view_connect_save": t_setup}}
+            if args.push_pull_every:
+                line["config"]["push_pull_every"] = args.push_pull_every
+                line["push_pull"] = res["push_pull"]
             print(json.dumps(line), flush=True)
     sim.close()
     if world > 1:

@@ -223,6 +223,36 @@ __global__ void __launch_bounds__(kGT) radix_scatter_kernel(const uint32_t *kin,
   }
 }
 
+// Stable sort of the E keys of kin[0..cnt) that are not SWIM_NO_MEMBER (all < N), ascending; an element's value is its
+// position / cap. *key / *val point into scratch of `s`.
+int sort_by_key(swim_sim *sim, Scratch &s, const uint32_t *kin, size_t cnt, uint32_t cap, u64 E, uint32_t N, const uint32_t **key,
+                const uint32_t **val) {
+  uint32_t *kb[2], *vb[2], *hist;
+  u64 *off;
+  for (int b = 0; b < 2; ++b) { SCRATCH(s, kb[b], E); SCRATCH(s, vb[b], E); }
+  const uint32_t T0 = (uint32_t)((cnt + kTile - 1) / kTile);
+  SCRATCH(s, hist, (size_t)256 * T0);
+  SCRATCH(s, off, (size_t)256 * T0 + 1);
+  const uint32_t bits = 32 - __builtin_clz(N - 1); // N >= 2 here: no key exists otherwise
+  const uint32_t *vin = nullptr;
+  int rc;
+  for (uint32_t pass = 0; pass * 8 < bits; ++pass) {
+    const uint32_t T = (uint32_t)((cnt + kTile - 1) / kTile), g = (uint32_t)grid_of(sim, T);
+    SWIM_LAUNCH(radix_hist_kernel, g, kGT, sim->stream, kin, cnt, pass * 8, hist, T);
+    ++sim->launches;
+    if ((rc = scan_u32(sim, s, hist, (size_t)256 * T, off))) return rc;
+    SWIM_LAUNCH(radix_scatter_kernel, g, kGT, sim->stream, kin, vin, cap, cnt, pass * 8, (const u64 *)off, T, kb[pass & 1], vb[pass & 1]);
+    ++sim->launches;
+    GRAPH_TRY(sim, cudaGetLastError());
+    kin = kb[pass & 1];
+    vin = vb[pass & 1];
+    cnt = E;
+  }
+  *key = kin;
+  *val = vin;
+  return SWIM_OK;
+}
+
 // ------------------------------------------------------------------ the graph
 // Validation and degrees in one pass over the id matrix: deg[m] = senders listing m, ldeg[m] = this shard's rows listing
 // m (sharded only); bad[0] = first local slot that breaks "ascending ids != self, vacancies last" (check_local),
@@ -378,31 +408,7 @@ int build_graph(swim_sim *sim, const uint32_t *nbr, const char *api) {
   }
   // sort every edge of the matrix by receiver (stable: senders stay ascending)
   const uint32_t *key = nullptr, *val = nullptr;
-  if (E_all) {
-    uint32_t *kb[2], *vb[2], *hist;
-    u64 *off;
-    for (int b = 0; b < 2; ++b) { SCRATCH(s, kb[b], E_all); SCRATCH(s, vb[b], E_all); }
-    const uint32_t T0 = (uint32_t)((slots + kTile - 1) / kTile);
-    SCRATCH(s, hist, (size_t)256 * T0);
-    SCRATCH(s, off, (size_t)256 * T0 + 1);
-    const uint32_t bits = 32 - __builtin_clz(N - 1); // N >= 2 here: a row never lists its own id
-    const uint32_t *kin = nbr, *vin = nullptr;
-    size_t cnt = slots;
-    for (uint32_t pass = 0; pass * 8 < bits; ++pass) {
-      const uint32_t T = (uint32_t)((cnt + kTile - 1) / kTile), g = (uint32_t)grid_of(sim, T);
-      SWIM_LAUNCH(radix_hist_kernel, g, kGT, sim->stream, kin, cnt, pass * 8, hist, T);
-      ++sim->launches;
-      if ((rc = scan_u32(sim, s, hist, (size_t)256 * T, off))) return rc;
-      SWIM_LAUNCH(radix_scatter_kernel, g, kGT, sim->stream, kin, vin, cap, cnt, pass * 8, (const u64 *)off, T, kb[pass & 1], vb[pass & 1]);
-      ++sim->launches;
-      GRAPH_TRY(sim, cudaGetLastError());
-      kin = kb[pass & 1];
-      vin = vb[pass & 1];
-      cnt = E_all;
-    }
-    key = kin;
-    val = vin;
-  }
+  if (E_all && (rc = sort_by_key(sim, s, nbr, slots, cap, E_all, N, &key, &val))) return rc;
   // the new index replaces the old one
   if (sim->d_in_src) { cudaFree(sim->d_in_src); sim->d_in_src = nullptr; }
   if (sim->d_eflag) { cudaFree(sim->d_eflag); sim->d_eflag = nullptr; }
@@ -492,6 +498,33 @@ __global__ void __launch_bounds__(kGT) remove_dead_kernel(SimDev d, uint32_t rou
   if (lane == 0 && removed) atomicAdd(n_removed, (u64)removed);
 }
 
+// Map.insert (Core.hs:206-216) on a row held by a warp (lane owns slots 32 w + lane), in registers: slots >= pos move up
+// by one (the last slot is vacant: the row is not full) and member m takes slot pos, Alive with incarnation inc0 and
+// lastChange = round. After the rotation lane l holds lane l - 1 of the same word; lane 0 takes lane 31 of the word before.
+template <int W>
+__device__ __forceinline__ void insert_slot(uint32_t (&nb)[W], uint32_t (&st)[W], uint32_t (&inc)[W], uint32_t (&last)[W],
+                                            uint32_t pos, uint32_t m, uint32_t inc0, uint32_t round, int lane) {
+  uint32_t up_nb[W], up_st[W], up_inc[W], up_last[W];
+  const int src = (lane + 31) & 31;
+#pragma unroll
+  for (int w = 0; w < W; ++w) {
+    up_nb[w] = __shfl_sync(kFull, nb[w], src); up_st[w] = __shfl_sync(kFull, st[w], src);
+    up_inc[w] = __shfl_sync(kFull, inc[w], src); up_last[w] = __shfl_sync(kFull, last[w], src);
+  }
+  if (lane == 0) {
+#pragma unroll
+    for (int w = W - 1; w >= 1; --w) {
+      up_nb[w] = up_nb[w - 1]; up_st[w] = up_st[w - 1]; up_inc[w] = up_inc[w - 1]; up_last[w] = up_last[w - 1];
+    }
+  }
+#pragma unroll
+  for (int w = 0; w < W; ++w) {
+    const uint32_t s = 32 * w + lane;
+    if (s == pos) { nb[w] = m; st[w] = SWIM_ALIVE; inc[w] = inc0; last[w] = round; }
+    else if (s > pos) { nb[w] = up_nb[w]; st[w] = up_st[w]; inc[w] = up_inc[w]; last[w] = up_last[w]; }
+  }
+}
+
 // addNewMember (Core.hs:206-216) for the observers of the adds: adds[grp[g] .. grp[g + 1]) are one observer's, in the
 // order given. A listed member is left alone; an unlisted one is inserted in id order as Alive with the add's
 // incarnation and lastChange = round; an add to a full row is dropped. res = {added, dropped on a full row}.
@@ -524,27 +557,7 @@ __global__ void __launch_bounds__(kGT) add_members_kernel(SimDev d, uint32_t rou
       }
       if (hit) continue;
       if (used == d.cap) { ++full; continue; }
-      // slots >= pos move up by one (the last slot is vacant: used < cap), the new member takes slot pos. After the
-      // rotation lane l holds lane l - 1 of the same word; lane 0 takes lane 31 of the word before.
-      uint32_t up_nb[W], up_st[W], up_inc[W], up_last[W];
-      const int src = (lane + 31) & 31;
-#pragma unroll
-      for (int w = 0; w < W; ++w) {
-        up_nb[w] = __shfl_sync(kFull, nb[w], src); up_st[w] = __shfl_sync(kFull, st[w], src);
-        up_inc[w] = __shfl_sync(kFull, inc[w], src); up_last[w] = __shfl_sync(kFull, last[w], src);
-      }
-      if (lane == 0) {
-#pragma unroll
-        for (int w = W - 1; w >= 1; --w) {
-          up_nb[w] = up_nb[w - 1]; up_st[w] = up_st[w - 1]; up_inc[w] = up_inc[w - 1]; up_last[w] = up_last[w - 1];
-        }
-      }
-#pragma unroll
-      for (int w = 0; w < W; ++w) {
-        const uint32_t s = 32 * w + lane;
-        if (s == pos) { nb[w] = m; st[w] = SWIM_ALIVE; inc[w] = ad.z; last[w] = round; }
-        else if (s > pos) { nb[w] = up_nb[w]; st[w] = up_st[w]; inc[w] = up_inc[w]; last[w] = up_last[w]; }
-      }
+      insert_slot<W>(nb, st, inc, last, pos, m, ad.z, round, lane);
       ++used;
       ++added;
       changed = true;

@@ -1,0 +1,209 @@
+// swim_pushpull.cuh — the push-pull state exchange between steps (DESIGN.md §2.6), on the device.
+// Compiled as part of swim_sim.cu's translation unit, after swim_graph.cuh (whose scan, sort, scratch and row-insert
+// helpers it uses).
+//
+// memberlist's periodic anti-entropy: every up node picks one random Alive member of its view, and if that partner is up
+// the two swap their full member state. Each side merges what it receives through the receive path's state machine
+// (row_apply), and a merge inserts the Alive members it did not list — the only way a bulk run learns unknown members.
+// Everything that is sent is read from a snapshot taken before any row changes, so the result does not depend on the
+// order in which warps run.
+#pragma once
+
+#include "swim_graph.cuh"
+
+namespace {
+
+// One thread per node: the partner p_i = the floor(x L / 2^32)-th Alive slot (ascending), x = word 0 of Philox block
+// (round, i, P_PUSHPULL, 0). part[i] = p_i if i and p_i are both up, else SWIM_NO_MEMBER; cnt[p_i] counts p_i's choosers.
+__global__ void __launch_bounds__(kGT) pp_pick_kernel(SimDev d, uint32_t round, uint32_t *part, uint32_t *cnt, u64 *n_ex) {
+  uint32_t ex = 0;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < d.n; i += gridDim.x * blockDim.x) {
+    uint32_t p = SWIM_NO_MEMBER;
+    if (d.alive[i]) {
+      const uint8_t *st = d.vst + (size_t)i * d.cap;
+      uint32_t L = 0;
+      for (uint32_t s = 0; s < d.cap; ++s) L += (st[s] & 3u) == SWIM_ALIVE;
+      if (L) {
+        uint32_t k = bounded(philox4x32_10(make_uint4(round, i, P_PUSHPULL, 0), d.key0, d.key1).x, L), s = 0;
+        for (;; ++s)
+          if ((st[s] & 3u) == SWIM_ALIVE && k-- == 0) break;
+        p = d.nbr[(size_t)i * d.cap + s];
+        if (d.alive[p]) { atomicAdd(&cnt[p], 1u); ++ex; }
+        else p = SWIM_NO_MEMBER;
+      }
+    }
+    part[i] = p;
+  }
+  ex = __reduce_add_sync(kFull, ex);
+  if ((threadIdx.x & 31) == 0 && ex) atomicAdd(n_ex, (u64)ex);
+}
+
+// The sender's state as the snapshot holds it.
+struct PpSnap {
+  const uint32_t *nbr, *vinc, *self_inc;
+  const uint8_t *vst;
+};
+
+// One warp per receiver j: senders {part[j]} ∪ choosers(j) in ascending id, each once; record by record through
+// row_apply (net), insertion of unknown Alive members, re-broadcast of every `Just`. res = {inserted, dropped on a full row}.
+template <int W>
+__global__ void __launch_bounds__(kThreads) push_pull_kernel(SimDev d, uint32_t round, PpSnap snap, const uint32_t *part,
+                                                             const u64 *seg, const uint32_t *chooser, u64 *res) {
+  SWIM_SHARED_2D(uint4, s_pb, kWarpsPerBlock, 32);
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  const uint32_t warp = blockIdx.x * kWarpsPerBlock + wib, nwarps = gridDim.x * kWarpsPerBlock;
+  Ctr c; c.clear();
+  PbStage pbs; pbs.s = s_pb[wib];
+  uint32_t inserted = 0, full = 0;
+  for (uint32_t j = warp; j < d.n; j += nwarps) {
+    uint32_t pull = part[j];
+    u64 x = seg[j];
+    const u64 x1 = seg[j + 1];
+    if (pull == SWIM_NO_MEMBER && x == x1) continue; // (a crashed node neither chooses nor is chosen)
+    Row<W> row;
+    row_load<W>(row, d, j, lane);
+    pb_load(pbs, d, j, lane);
+    uint32_t last[W], td[W], used = 0;
+#pragma unroll
+    for (int w = 0; w < W; ++w) {
+      last[w] = d.vlast[(size_t)j * d.cap + 32 * w + lane];
+      td[w] = d.meta[(size_t)j * W + w].z;
+      used += __popc(__ballot_sync(kFull, (row.st[w] & 3u) != SWIM_VACANT));
+    }
+    uint32_t self_inc = d.self_inc[j];
+    const uint32_t self_inc0 = self_inc;
+    bool grew = false;
+    for (;;) {
+      const uint32_t ch = x < x1 ? chooser[x] : SWIM_NO_MEMBER;
+      uint32_t s;
+      if (pull != SWIM_NO_MEMBER && pull <= ch) { s = pull; pull = SWIM_NO_MEMBER; if (ch == s) ++x; }
+      else if (ch != SWIM_NO_MEMBER) { s = ch; ++x; }
+      else break;
+      // the sender's row, lane-owned like the receiver's
+      uint32_t snb[W], sst[W], sinc[W];
+      int nocc = 0; // occupied slots (vacancies are last)
+#pragma unroll
+      for (int w = 0; w < W; ++w) {
+        const size_t y = (size_t)s * d.cap + 32 * w + lane;
+        snb[w] = snap.nbr[y]; sst[w] = snap.vst[y] & 3u; sinc[w] = snap.vinc[y];
+        nocc += __popc(__ballot_sync(kFull, sst[w] != SWIM_VACANT));
+      }
+      // record -1: Alive(self_inc, s); then one per occupied slot, in slot order
+      for (int q = -1; q < nocc; ++q) {
+        uint4 rec;
+        if (q < 0) {
+          rec = make_rec(s, snap.self_inc[s], 0, SWIM_MSG_ALIVE);
+        } else {
+          uint32_t m = 0, lv = 0, vi = 0;
+#pragma unroll
+          for (int w = 0; w < W; ++w) {
+            const uint32_t a = __shfl_sync(kFull, snb[w], q & 31), b = __shfl_sync(kFull, sst[w], q & 31),
+                           e = __shfl_sync(kFull, sinc[w], q & 31);
+            if (w == (q >> 5)) { m = a; lv = b; vi = e; }
+          }
+          rec = make_rec(m, vi, lv == SWIM_DEAD ? s : 0u,
+                         lv == SWIM_ALIVE ? SWIM_MSG_ALIVE : lv == SWIM_SUSPECT ? SWIM_MSG_SUSPECT : SWIM_MSG_DEAD);
+        }
+        uint4 rb;
+        const int v = row_apply<W>(row, d, j, self_inc, rec, rb, lane, c.v[SWIM_CTR_REFUTES]);
+        if (v == 2) { // an Alive member j does not list: addNewMember (Core.hs:206-216), as swim_alive_node inserts
+          if (used == d.cap) { ++full; continue; }
+          uint32_t pos = 0;
+#pragma unroll
+          for (int w = 0; w < W; ++w) {
+            pos += __popc(__ballot_sync(kFull, (row.st[w] & 3u) != SWIM_VACANT && row.nb[w] < rec.x));
+            if (row.touched >> w & 1u) last[w] = round; // slots change places: lastChange moves with them
+          }
+          row.touched = 0;
+          insert_slot<W>(row.nb, row.st, row.inc, last, pos, rec.x, rec.y, round, lane);
+          ++used;
+          ++inserted;
+          grew = true;
+          rb = rec;
+        } else if (v != 1) {
+          continue;
+        }
+        pb_enqueue(pbs, d, rb, lane, c.v[SWIM_CTR_PB_DROPPED]);
+        if (lane == 0) ++c.v[SWIM_CTR_RECS_APPLIED];
+      }
+    }
+    if (grew) { // slots moved: the whole row is written (the per-node records are re-derived before the next round)
+#pragma unroll
+      for (int w = 0; w < W; ++w) {
+        const size_t y = (size_t)j * d.cap + 32 * w + lane;
+        if (row.touched >> w & 1u) last[w] = round;
+        d.nbr[y] = row.nb[w]; d.vst[y] = (uint8_t)row.st[w]; d.vinc[y] = row.inc[w]; d.vlast[y] = last[w];
+      }
+    } else {
+      row_store<W>(row, d, j, lane, round, td);
+    }
+    pb_store(pbs, d, j, lane);
+    if (lane == 0 && self_inc != self_inc0) d.self_inc[j] = self_inc;
+  }
+  if (lane == 0 && (inserted || full)) { atomicAdd(&res[0], (u64)inserted); atomicAdd(&res[1], (u64)full); }
+  c.flush(d.ctr, lane);
+}
+
+} // namespace
+
+extern "C" int swim_sim_push_pull(swim_sim_t *sim, uint64_t *n_exchanges, uint64_t *n_inserted, uint64_t *n_full) {
+  if (!sim) return SWIM_EINVAL;
+  const SimDev &d = sim->dev;
+  if (d.world != 1) { set_error(sim, "swim_sim_push_pull: single shard only (a partner's row may live on another rank)"); return SWIM_ESTATE; }
+  if (!sim->view_set) { set_error(sim, "swim_sim_push_pull: no view installed"); return SWIM_ESTATE; }
+  if (sim->failed) { set_error(sim, "swim_sim_push_pull: an earlier step failed part-way; the handle's device state is undefined"); return SWIM_ESTATE; }
+  cudaSetDevice(sim->device);
+  const size_t n = d.n, slots = n * d.cap;
+  Scratch s(sim);
+  uint32_t *part, *cnt;
+  u64 *seg, *res, h[3] = {0, 0, 0}, E = 0;
+  SCRATCH(s, part, n);
+  SCRATCH(s, cnt, n);
+  SCRATCH(s, seg, n + 1);
+  SCRATCH(s, res, 3);
+  GRAPH_TRY(sim, cudaMemsetAsync(cnt, 0, n * 4, sim->stream));
+  GRAPH_TRY(sim, cudaMemsetAsync(res, 0, 3 * 8, sim->stream));
+  SWIM_LAUNCH(pp_pick_kernel, grid_of(sim, (n + kGT - 1) / kGT), kGT, sim->stream, d, sim->round, part, cnt, res + 2);
+  ++sim->launches;
+  GRAPH_TRY(sim, cudaGetLastError());
+  int rc;
+  if ((rc = scan_u32(sim, s, cnt, n, seg))) return rc;
+  GRAPH_TRY(sim, cudaMemcpyAsync(&E, seg + n, 8, cudaMemcpyDeviceToHost, sim->stream));
+  GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
+  if (E) {
+    // the choosers of every node, ascending: a stable sort of the partner array by partner
+    const uint32_t *key, *chooser;
+    if ((rc = sort_by_key(sim, s, part, n, 1, E, d.N, &key, &chooser))) return rc;
+    PpSnap snap;
+    uint32_t *nb, *vi, *si;
+    uint8_t *vs;
+    SCRATCH(s, nb, slots);
+    SCRATCH(s, vi, slots);
+    SCRATCH(s, si, n);
+    SCRATCH(s, vs, slots);
+    GRAPH_TRY(sim, cudaMemcpyAsync(nb, d.nbr, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
+    GRAPH_TRY(sim, cudaMemcpyAsync(vi, d.vinc, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
+    GRAPH_TRY(sim, cudaMemcpyAsync(si, d.self_inc, n * 4, cudaMemcpyDeviceToDevice, sim->stream));
+    GRAPH_TRY(sim, cudaMemcpyAsync(vs, d.vst, slots, cudaMemcpyDeviceToDevice, sim->stream));
+    snap.nbr = nb; snap.vinc = vi; snap.self_inc = si; snap.vst = vs;
+    const int g = grid_of(sim, (n + kWarpsPerBlock - 1) / kWarpsPerBlock);
+    const uint32_t *cp = part;
+    const u64 *cs = seg;
+    switch (d.cap / 32) {
+      case 1: SWIM_LAUNCH(push_pull_kernel<1>, g, kThreads, sim->stream, d, sim->round, snap, cp, cs, chooser, res); break;
+      case 2: SWIM_LAUNCH(push_pull_kernel<2>, g, kThreads, sim->stream, d, sim->round, snap, cp, cs, chooser, res); break;
+      case 4: SWIM_LAUNCH(push_pull_kernel<4>, g, kThreads, sim->stream, d, sim->round, snap, cp, cs, chooser, res); break;
+      default: SWIM_LAUNCH(push_pull_kernel<8>, g, kThreads, sim->stream, d, sim->round, snap, cp, cs, chooser, res); break;
+    }
+    ++sim->launches;
+    GRAPH_TRY(sim, cudaGetLastError());
+  }
+  GRAPH_TRY(sim, cudaMemcpyAsync(h, res, sizeof h, cudaMemcpyDeviceToHost, sim->stream));
+  GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
+  if (h[0]) mark_edited(sim); // members were inserted: the mail graph is rebuilt by the next step
+  else sim->tdead_dirty = true;
+  if (n_exchanges) *n_exchanges = h[2];
+  if (n_inserted) *n_inserted = h[0];
+  if (n_full) *n_full = h[1];
+  return SWIM_OK;
+}

@@ -301,6 +301,8 @@ extern "C" int swim_sim_local_range(const swim_sim_t *sim, uint32_t *first, uint
 
 // swim_sim_set_view / _set_view_device, the device-side mail-graph build and the bulk membership edits
 #include "swim_graph.cuh"
+// swim_sim_push_pull: the state exchange between steps
+#include "swim_pushpull.cuh"
 
 // ------------------------------------------------------------------ events
 extern "C" int swim_sim_inject(swim_sim_t *sim, const swim_event_t *ev, size_t n) {

@@ -154,6 +154,14 @@ class Simulator:
               "swim_sim_add_members", self._h)
         return added.value, full.value
 
+    def push_pull(self):
+        """Push-pull state exchange (DESIGN.md 2.6) at the current round: every up node swaps its full member state with
+        one random Alive member, and each side merges what it receives, inserting the Alive members it did not list.
+        Single shard. Returns (exchanges, inserted, full)."""
+        e, n, f = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        check(lib().swim_sim_push_pull(self._h, C.byref(e), C.byref(n), C.byref(f)), "swim_sim_push_pull", self._h)
+        return e.value, n.value, f.value
+
     def inject(self, events):
         events = np.ascontiguousarray(events, dtype=A.EVENT_DTYPE)
         check(lib().swim_sim_inject(self._h, events.ctypes.data, len(events)), "swim_sim_inject", self._h)

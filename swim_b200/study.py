@@ -94,20 +94,28 @@ def latency_stats(hist):
             "max": int(np.flatnonzero(hist)[-1])}
 
 
-def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None):
+def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None, push_pull_every=0):
     """Step `rounds` rounds, sampling the convergence count; returns the time series, the final counters and the final
-    view report. `reduce_sum(list_of_numbers) -> list` adds values over ranks (identity for one GPU)."""
+    view report. `reduce_sum(list_of_numbers) -> list` adds values over ranks (identity for one GPU). push_pull_every = R
+    > 0: a push-pull state exchange (Simulator.push_pull, single shard) after every R-th round; its summed outputs are
+    in "push_pull"."""
     red = reduce_sum or (lambda xs: xs)
     series = []
     done = 0
     device_ms = 0.0
+    pp = [0, 0, 0]
     while done < rounds:
-        step = min(sample_every, rounds - done)
+        step = min(sample_every - done % sample_every, rounds - done)
+        if push_pull_every:
+            step = min(step, push_pull_every - done % push_pull_every)
         sim.step(step)
         if hasattr(sim, "last_step_ms"):
             device_ms += float(sim.last_step_ms())  # CUDA events around the call's kernels, this rank
         done += step
-        series.append((done, int(red([sim.mismatches()])[0])))
+        if push_pull_every and done % push_pull_every == 0:
+            pp = [a + b for a, b in zip(pp, sim.push_pull())]
+        if done % sample_every == 0 or done == rounds:
+            series.append((done, int(red([sim.mismatches()])[0])))
     counters = [int(x) for x in red([int(v) for v in sim.counters()])]
     rep = view_report(sim, events, done)
     hist = np.array(red(rep.pop("latency_hist").tolist()), dtype=np.int64)
@@ -115,5 +123,8 @@ def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None):
     vals = red([rep[k] for k in keys])
     rep = dict(zip(keys, (int(v) for v in vals)))
     rep["latency"] = latency_stats(hist)
-    return {"mismatch_series": series, "counters": dict(zip(A.CTR_NAMES, counters)), "report": rep,
-            "device_ms": device_ms, "device_us_per_round": device_ms * 1e3 / max(1, rounds)}
+    out = {"mismatch_series": series, "counters": dict(zip(A.CTR_NAMES, counters)), "report": rep,
+           "device_ms": device_ms, "device_us_per_round": device_ms * 1e3 / max(1, rounds)}
+    if push_pull_every:
+        out["push_pull"] = dict(zip(("exchanges", "inserted", "full"), pp))
+    return out
