@@ -305,10 +305,13 @@ int swim_sim_load(swim_sim_t *sim);
  * parameter sweep on ONE handle: the view, its in-edge index and the device arrays are built once. */
 int swim_sim_set_params(swim_sim_t *sim, const swim_config_t *cfg);
 
-/* Bulk membership edits between steps, on the device (one warp per affected row, no host copy of the rows). Single
- * shard only (SWIM_ESTATE when world > 1). Both mark the view changed: the next step rebuilds the in-edge index, the
- * checkpoint is dropped (swim_sim_load fails until the next swim_sim_save), and swim_sim_export_round returns
- * SWIM_ESTATE until the next step.
+/* Bulk membership edits between steps, on the device (one warp per affected row, no host copy of the rows). Both mark
+ * the view changed: the next step rebuilds the in-edge index, the checkpoint is dropped (swim_sim_load fails until the
+ * next swim_sim_save), and swim_sim_export_round returns SWIM_ESTATE until the next step. On a sharded handle (world > 1)
+ * they are collectives, like swim_sim_push_pull and swim_sim_load: every rank issues the same calls in the same order
+ * (swim_sim_add_members with the same global list; each rank applies its own observers' adds), outputs are this
+ * rank's counts, and the next step rebuilds the index on all ranks together; SWIM_ESTATE before swim_sim_ipc_connect /
+ * swim_sim_connect. Scalar membership changes on a sharded handle still make its next step return SWIM_ESTATE.
  *
  * removeDeadNodes (Core.hs:65-67) on every local store at once: Dead entries with round - last_change >= min_age leave
  * (round = rounds executed so far; min_age = 0 is the reference's form, swim_remove_dead_nodes on every node). Rows stay
@@ -331,9 +334,11 @@ int swim_sim_add_members(swim_sim_t *sim, const swim_member_add_t *adds, size_t 
  * (Alive(self), then every occupied slot as Alive / Suspect / Dead(from = sender)), read from a snapshot taken before
  * anything changes. A receiver merges its senders in ascending id, each record through the receive rules; an Alive record
  * about a member it does not list is inserted as swim_alive_node inserts (aliveNode / addNewMember, Core.hs:206-216), and
- * dropped when the row is full. Two calls at the same round pick the same partners. No message is lost. Single shard
- * only; SWIM_ESTATE when world > 1, before a view is installed and on a failed handle. Without inserts only state
- * changes and the checkpoint stays valid; with inserts the view is marked changed as by the bulk edits above.
+ * dropped when the row is full. Two calls at the same round pick the same partners. No message is lost. On a sharded
+ * handle a collective (every rank calls it; outputs are this rank's, their sums the single-shard ones); SWIM_ESTATE on
+ * a sharded handle that is not connected, before a view is installed and on a failed handle. Without inserts only state
+ * changes and the checkpoint stays valid; with inserts (on any rank) the view is marked changed as by the bulk edits
+ * above.
  * Outputs may be NULL: *n_exchanges = choices whose partner was up, *n_inserted = members inserted, *n_full = inserts
  * dropped on a full row. */
 int swim_sim_push_pull(swim_sim_t *sim, uint64_t *n_exchanges, uint64_t *n_inserted, uint64_t *n_full);

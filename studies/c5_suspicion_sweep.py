@@ -37,7 +37,8 @@ def main():
     ap.add_argument("--topology", default="random", choices=["random", "ring"])
     ap.add_argument("--sample-every", type=int, default=10)
     ap.add_argument("--push-pull-every", type=int, default=0, metavar="R",
-                    help="a push-pull state exchange (memberlist anti-entropy) after every R-th round; one GPU only")
+                    help="a push-pull state exchange (memberlist anti-entropy) after every R-th round (a collective "
+                         "on several GPUs)")
     ap.add_argument("--seed", type=int, default=0x5EED0001 + 5)
     args = ap.parse_args()
 
@@ -47,9 +48,6 @@ def main():
     from swim_b200.study import run_sweep_point
 
     rank, world, local = sd.init_from_env()
-    if args.push_pull_every and world > 1:
-        raise SystemExit("--push-pull-every needs one GPU: the exchange reads partners' rows, which live on other ranks "
-                         "when the simulation is sharded")
     if not torch.cuda.is_available():
         raise SystemExit("c5_suspicion_sweep needs a CUDA device (there is no CPU fallback)")
     torch.cuda.set_device(local)

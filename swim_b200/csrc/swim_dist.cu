@@ -15,8 +15,11 @@
 #include <nccl.h>
 
 #include <algorithm>
+#include <chrono>
+#include <cstddef>
 #include <cstdlib>
 #include <cstring>
+#include <thread>
 #include <vector>
 
 #include "swim_host.h"
@@ -159,17 +162,22 @@ extern "C" int swim_sim_connect(swim_sim_t *sim, const uint8_t *id) {
 
 // ------------------------------------------------------------------ fused exchange over peer memory
 namespace {
+// Arrays a rank exports: the round kernels' (eflag .. mailbits) and what the collectives between steps read (nbr .. coll).
+// None of them changes size with the view: eflag is the only view-sized array a peer maps, and a sharded rebuild re-maps
+// it (coll_remap_eflag); out, out_cnt, rlr, rcnt, bar and mailbits are sized from `per` / `rcap`, nbr, vst, vinc and
+// self_inc from the shard's rows.
+enum { kXEflag, kXOut, kXOutCnt, kXRlr, kXRcnt, kXBar, kXMailbits, kXNbr, kXVst, kXVinc, kXSelfInc, kXColl, kXCount };
 struct IpcBlob {
   uint32_t magic, rank, n, estride;
-  cudaIpcMemHandle_t h[7]; // eflag, out, out_cnt, rlr, rcnt, bar, mailbits
+  cudaIpcMemHandle_t h[kXCount];
   // the exporting process and its raw device pointers: ranks that live in ONE process (several handles, on one device or
   // on peer devices) cannot open each other's IPC handles — they use the pointers as they are
   uint64_t pid;
   int32_t device, _pad;
-  uint64_t raw[7];
+  uint64_t raw[kXCount];
 };
 static_assert(sizeof(IpcBlob) <= SWIM_IPC_BLOB_BYTES, "blob too small");
-constexpr uint32_t kBlobMagic = 0x53574D49u; // "SWMI"
+constexpr uint32_t kBlobMagic = 0x53574D4Au; // "SWMJ"
 } // namespace
 
 extern "C" int swim_sim_ipc_export(swim_sim_t *sim, uint8_t *blob) {
@@ -180,8 +188,9 @@ extern "C" int swim_sim_ipc_export(swim_sim_t *sim, uint8_t *blob) {
   IpcBlob b;
   memset(&b, 0, sizeof b);
   b.magic = kBlobMagic; b.rank = d.rank; b.n = d.n; b.estride = d.estride;
-  void *ptrs[7] = {d.eflag, d.out, d.out_cnt, d.rlr, d.rcnt, sim->d_bar, d.mailbits};
-  for (int x = 0; x < 7; ++x) {
+  void *ptrs[kXCount] = {d.eflag, d.out, d.out_cnt, d.rlr, d.rcnt, sim->d_bar, d.mailbits,
+                         d.nbr, d.vst, d.vinc, d.self_inc, sim->d_coll};
+  for (int x = 0; x < kXCount; ++x) {
     CUDA_TRY(sim, cudaIpcGetMemHandle(&b.h[x], ptrs[x]));
     b.raw[x] = (uint64_t)(uintptr_t)ptrs[x];
   }
@@ -203,24 +212,28 @@ extern "C" int swim_sim_ipc_connect(swim_sim_t *sim, const uint8_t *blobs) {
     memcpy(&b, blobs + (size_t)r * SWIM_IPC_BLOB_BYTES, sizeof b);
     if (b.magic != kBlobMagic || b.rank != r) { set_error(sim, "swim_sim_ipc_connect: blob %u is not rank %u's export", r, r); return SWIM_EINVAL; }
     if (r == d.rank) continue;
-    void *p[7];
-    if (b.pid == (uint64_t)getpid()) { // a rank of this very process: its pointers are valid here as they are
+    void *p[kXCount];
+    sim->peer.same_process[r] = b.pid == (uint64_t)getpid();
+    if (sim->peer.same_process[r]) { // a rank of this very process: its pointers are valid here as they are
       if (b.device != sim->device) {
         cudaError_t e = cudaDeviceEnablePeerAccess(b.device, 0);
         if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) { set_error(sim, "swim_sim_ipc_connect: no peer access to device %d: %s", b.device, cudaGetErrorString(e)); return SWIM_ECUDA; }
         cudaGetLastError();
       }
-      for (int x = 0; x < 7; ++x) p[x] = (void *)(uintptr_t)b.raw[x];
+      for (int x = 0; x < kXCount; ++x) p[x] = (void *)(uintptr_t)b.raw[x];
     } else {
-      for (int x = 0; x < 7; ++x) {
+      for (int x = 0; x < kXCount; ++x) {
         CUDA_TRY(sim, cudaIpcOpenMemHandle(&p[x], b.h[x], cudaIpcMemLazyEnablePeerAccess));
         sim->ipc_opened.push_back(p[x]);
       }
     }
-    d.eflag_p[r] = (uint8_t *)p[0]; d.estride_p[r] = b.estride;
-    d.out_p[r] = (const uint4 *)p[1]; d.out_cnt_p[r] = (const uint8_t *)p[2];
-    d.rlr_p[r] = (uint32_t *)p[3]; d.rcnt_p[r] = (uint32_t *)p[4]; d.bar_p[r] = (uint32_t *)p[5];
-    d.mailbits_p[r] = (uint32_t *)p[6];
+    d.eflag_p[r] = (uint8_t *)p[kXEflag]; d.estride_p[r] = b.estride;
+    d.out_p[r] = (const uint4 *)p[kXOut]; d.out_cnt_p[r] = (const uint8_t *)p[kXOutCnt];
+    d.rlr_p[r] = (uint32_t *)p[kXRlr]; d.rcnt_p[r] = (uint32_t *)p[kXRcnt]; d.bar_p[r] = (uint32_t *)p[kXBar];
+    d.mailbits_p[r] = (uint32_t *)p[kXMailbits];
+    PeerViews &v = sim->peer;
+    v.nbr[r] = (const uint32_t *)p[kXNbr]; v.vst[r] = (const uint8_t *)p[kXVst]; v.vinc[r] = (const uint32_t *)p[kXVinc];
+    v.self_inc[r] = (const uint32_t *)p[kXSelfInc]; v.coll[r] = (CollBlock *)p[kXColl];
   }
   d.p2p = 1;
   sim->connected = true;
@@ -290,6 +303,161 @@ int dist_exchange(swim_sim *sim) {
   SWIM_LAUNCH(deliver_kernel, grid, 256, sim->stream, d, da, (uint32_t)total_recv);
   ++sim->launches;
   return SWIM_OK;
+}
+
+} // namespace swim
+
+// ------------------------------------------------------------------ collectives between steps
+// The sharded forms of the bulk membership calls and of the mail-graph rebuild (swim_graph.cuh, swim_pushpull.cuh) need
+// three things from the peers while no round runs: a barrier, which may carry one value per rank and return their sum; a
+// gather of one per-row array into a [world x per]-row buffer (rank r's rows from row r * per on, so the buffer is
+// addressed by global id and only its tail past N is padding); and, after a rebuild reallocated the mail flags, the
+// peers' new flag arrays. Over peer memory they use the arrays swim_sim_ipc_connect mapped and a barrier word of their
+// own (never the round kernels' words, whose handshake state must stay as it is); on the staged path, NCCL.
+namespace {
+struct CollPeers {
+  CollBlock *b[SWIM_MAX_WORLD];
+};
+
+// Thread q stores this rank's value into peer q's block, then (release, system scope) this barrier's generation.
+__global__ void coll_publish_kernel(uint32_t world, uint32_t rank, CollPeers p, uint32_t gen, unsigned long long val) {
+  const uint32_t q = threadIdx.x;
+  if (q < world && q != rank) {
+    __threadfence_system(); // this rank's writes before the barrier (its earlier kernels and copies) come first
+    p.b[q]->val[gen & 1][rank] = val;
+    st_release_sys(&p.b[q]->bar[rank], gen);
+  }
+}
+
+// Thread q reads (acquire) peer q's generation word in this rank's block and the value q brought with it.
+__global__ void coll_poll_kernel(uint32_t world, uint32_t rank, CollBlock *mine, uint32_t gen) {
+  const uint32_t q = threadIdx.x;
+  if (q < world && q != rank) {
+    const uint32_t g = ld_acquire_sys(&mine->bar[q]);
+    mine->seen[q] = g;
+    if ((int32_t)(g - gen) >= 0) mine->got[q] = *(volatile unsigned long long *)&mine->val[gen & 1][q];
+  }
+}
+
+// The wait of a barrier over peer memory is the host's, one short poll kernel at a time, and not a kernel spinning on
+// the device: ranks that share a device would otherwise dead-lock whenever one of them calls cudaFree (which waits for
+// every kernel on the device, the peer's spinning barrier included) before it reaches the barrier. The wait is bounded
+// like the round handshake's (about a minute).
+constexpr double kCollWaitSeconds = 60.0;
+} // namespace
+
+namespace swim {
+
+int coll_barrier(swim_sim *sim, unsigned long long mine, unsigned long long *sum) {
+  SimDev &d = sim->dev;
+  const uint32_t G = d.world;
+  unsigned long long got[SWIM_MAX_WORLD];
+  unsigned long long *d_got = (unsigned long long *)((uint8_t *)sim->d_coll + offsetof(CollBlock, got));
+  const uint32_t gen = ++sim->coll_gen;
+  if (d.p2p) {
+    CollPeers p;
+    memset(&p, 0, sizeof p);
+    for (uint32_t q = 0; q < G; ++q) p.b[q] = sim->peer.coll[q];
+    SWIM_LAUNCH(coll_publish_kernel, 1, 32, sim->stream, G, d.rank, p, gen, mine);
+    ++sim->launches;
+    CUDA_TRY(sim, cudaGetLastError());
+    const uint32_t *d_seen = (const uint32_t *)((const uint8_t *)sim->d_coll + offsetof(CollBlock, seen));
+    const auto t0 = std::chrono::steady_clock::now();
+    for (int poll = 0;; ++poll) {
+      uint32_t seen[SWIM_MAX_WORLD];
+      SWIM_LAUNCH(coll_poll_kernel, 1, 32, sim->stream, G, d.rank, sim->d_coll, gen);
+      ++sim->launches;
+      CUDA_TRY(sim, cudaGetLastError());
+      CUDA_TRY(sim, cudaMemcpyAsync(seen, d_seen, G * sizeof(uint32_t), cudaMemcpyDeviceToHost, sim->stream));
+      CUDA_TRY(sim, cudaMemcpyAsync(got, d_got, G * sizeof(unsigned long long), cudaMemcpyDeviceToHost, sim->stream));
+      CUDA_TRY(sim, cudaStreamSynchronize(sim->stream));
+      bool all = true;
+      for (uint32_t q = 0; q < G; ++q) all &= q == d.rank || (int32_t)(seen[q] - gen) >= 0;
+      if (all) break;
+      if (std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() > kCollWaitSeconds) {
+        set_error(sim, "a barrier between steps timed out (a peer rank did not make the same call)");
+        sim->failed = true;
+        return SWIM_ESTATE;
+      }
+      if (poll >= 16) std::this_thread::sleep_for(std::chrono::microseconds(50));
+    }
+  } else { // staged path: a one-word all-gather is the barrier
+    Dist *x = (Dist *)sim->dist;
+    if (!x) { set_error(sim, "multi-shard exchange not connected"); return SWIM_ESTATE; }
+    unsigned long long *w = d_got;
+    CUDA_TRY(sim, cudaMemcpyAsync(w + d.rank, &mine, sizeof mine, cudaMemcpyHostToDevice, sim->stream));
+    NCCL_TRY(sim, g_nccl.AllGather(w + d.rank, w, 1, ncclUint64, x->comm, sim->stream));
+    CUDA_TRY(sim, cudaMemcpyAsync(got, w, G * sizeof(unsigned long long), cudaMemcpyDeviceToHost, sim->stream));
+    CUDA_TRY(sim, cudaStreamSynchronize(sim->stream));
+  }
+  got[d.rank] = mine;
+  if (sum) {
+    *sum = 0;
+    for (uint32_t q = 0; q < G; ++q) *sum += got[q];
+  }
+  return SWIM_OK;
+}
+
+int coll_gather(swim_sim *sim, CollArray which, void *out) {
+  SimDev &d = sim->dev;
+  const size_t rb = which == kCollNbr || which == kCollVinc ? (size_t)d.cap * 4 : which == kCollVst ? d.cap : 4;
+  const void *local = which == kCollNbr ? (const void *)d.nbr : which == kCollVst ? (const void *)d.vst
+                    : which == kCollVinc ? (const void *)d.vinc : (const void *)d.self_inc;
+  uint8_t *o = (uint8_t *)out;
+  if (d.n) CUDA_TRY(sim, cudaMemcpyAsync(o + (size_t)d.rank * d.per * rb, local, d.n * rb, cudaMemcpyDeviceToDevice, sim->stream));
+  if (d.p2p) {
+    const PeerViews &v = sim->peer;
+    for (uint32_t r = 0; r < d.world; ++r) {
+      const uint32_t f = shard_first(d.N, d.world, r), n = shard_first(d.N, d.world, r + 1) - f;
+      if (r == d.rank || !n) continue;
+      const void *src = which == kCollNbr ? (const void *)v.nbr[r] : which == kCollVst ? (const void *)v.vst[r]
+                      : which == kCollVinc ? (const void *)v.vinc[r] : (const void *)v.self_inc[r];
+      CUDA_TRY(sim, cudaMemcpyAsync(o + (size_t)r * d.per * rb, src, n * rb, cudaMemcpyDefault, sim->stream));
+    }
+  } else {
+    Dist *x = (Dist *)sim->dist;
+    if (!x) { set_error(sim, "multi-shard exchange not connected"); return SWIM_ESTATE; }
+    const size_t part = (size_t)d.per * rb; // (in place: this rank's part of the buffer is its send buffer)
+    NCCL_TRY(sim, g_nccl.AllGather(o + d.rank * part, o, part, ncclUint8, x->comm, sim->stream));
+  }
+  CUDA_TRY(sim, cudaStreamSynchronize(sim->stream));
+  return SWIM_OK;
+}
+
+// After a sharded rebuild over peer memory: every rank's mail flags live in a new array with a new parity stride. Each
+// rank publishes its own in its block; after a barrier it maps every peer's (closing the old mapping); after a second
+// barrier nobody holds the retired arrays any more, and each rank frees its own. A third barrier follows the free: no
+// rank starts its round kernels (which wait for the peers on the device) while a peer that shares its device may still
+// be in cudaFree (which waits for every kernel on the device).
+int coll_remap_eflag(swim_sim *sim, uint8_t *retired) {
+  SimDev &d = sim->dev;
+  CollBlock pub;
+  memset(&pub, 0, sizeof pub);
+  CUDA_TRY(sim, cudaIpcGetMemHandle(&pub.eflag_h, d.eflag));
+  pub.eflag_raw = (unsigned long long)(uintptr_t)d.eflag;
+  pub.estride = d.estride;
+  const size_t off = offsetof(CollBlock, eflag_h), bytes = sizeof(CollBlock) - off;
+  CUDA_TRY(sim, cudaMemcpyAsync((uint8_t *)sim->d_coll + off, (const uint8_t *)&pub + off, bytes, cudaMemcpyHostToDevice, sim->stream));
+  CUDA_TRY(sim, cudaStreamSynchronize(sim->stream));
+  int rc;
+  if ((rc = coll_barrier(sim))) return rc;
+  for (uint32_t r = 0; r < d.world; ++r) {
+    if (r == d.rank) continue;
+    CollBlock b;
+    CUDA_TRY(sim, cudaMemcpy((uint8_t *)&b + off, (const uint8_t *)sim->peer.coll[r] + off, bytes, cudaMemcpyDefault));
+    void *p = (void *)(uintptr_t)b.eflag_raw;
+    if (!sim->peer.same_process[r]) {
+      auto it = std::find(sim->ipc_opened.begin(), sim->ipc_opened.end(), (void *)d.eflag_p[r]);
+      if (it != sim->ipc_opened.end()) { cudaIpcCloseMemHandle(*it); sim->ipc_opened.erase(it); }
+      CUDA_TRY(sim, cudaIpcOpenMemHandle(&p, b.eflag_h, cudaIpcMemLazyEnablePeerAccess));
+      sim->ipc_opened.push_back(p);
+    }
+    d.eflag_p[r] = (uint8_t *)p;
+    d.estride_p[r] = b.estride;
+  }
+  if ((rc = coll_barrier(sim))) return rc;
+  if (retired) CUDA_TRY(sim, cudaFree(retired));
+  return coll_barrier(sim);
 }
 
 void dist_teardown(swim_sim *sim) {

@@ -5,8 +5,9 @@
 // uses (obs_off / obs_slot) and the membership filters of all N rows are functions of the global id matrix alone.
 // build_graph derives them from a copy of that matrix in device memory: swim_sim_set_view (after one upload),
 // swim_sim_set_view_device (the caller's device buffer) and the first step after a membership change (the rows in
-// SimDev::nbr, single shard). The edges are taken in (sender, slot) order and sorted by receiver with a stable LSD
-// radix sort, so every receiver's senders come out ascending whatever its in-degree.
+// SimDev::nbr on one shard; on several, every rank's rows gathered into one matrix). The edges are taken in (sender,
+// slot) order and sorted by receiver with a stable LSD radix sort, so every receiver's senders come out ascending
+// whatever its in-degree.
 #pragma once
 #include <algorithm>
 #include <vector>
@@ -348,8 +349,9 @@ __global__ void __launch_bounds__(kGT) bloom_kernel(const uint32_t *nbr, uint32_
 }
 
 // The mail graph of the global id matrix `nbr` (device memory, [N * cap]). With `api` (swim_sim_set_view /
-// _set_view_device) the local rows are validated first and then installed, every member Alive at incarnation 0.
-int build_graph(swim_sim *sim, const uint32_t *nbr, const char *api) {
+// _set_view_device) the local rows are validated first and then installed, every member Alive at incarnation 0. With
+// `retired`, the old mail-flag array is handed back there instead of freed (peers may still have it mapped).
+int build_graph(swim_sim *sim, const uint32_t *nbr, const char *api, uint8_t **retired = nullptr) {
   SimDev &d = sim->dev;
   const uint32_t N = d.N, cap = d.cap;
   const size_t slots = (size_t)N * cap, lslots = (size_t)d.n * cap;
@@ -411,7 +413,9 @@ int build_graph(swim_sim *sim, const uint32_t *nbr, const char *api) {
   if (E_all && (rc = sort_by_key(sim, s, nbr, slots, cap, E_all, N, &key, &val))) return rc;
   // the new index replaces the old one
   if (sim->d_in_src) { cudaFree(sim->d_in_src); sim->d_in_src = nullptr; }
-  if (sim->d_eflag) { cudaFree(sim->d_eflag); sim->d_eflag = nullptr; }
+  if (retired) *retired = sim->d_eflag;
+  else if (sim->d_eflag) cudaFree(sim->d_eflag);
+  sim->d_eflag = nullptr;
   if (sim->d_bloom) { cudaFree(sim->d_bloom); sim->d_bloom = nullptr; }
   const size_t Ea = E ? (size_t)E : 1;
   const size_t estride = (Ea + 255) & ~(size_t)255; // parity stride of the mail flags
@@ -444,7 +448,7 @@ int install_view(swim_sim *sim, const uint32_t *nbr_dev, const char *api) {
   int rc = build_graph(sim, nbr_dev, api);
   if (rc) return rc;
   sim->view_set = true;
-  sim->edges_dirty = false;
+  sim->edges_dirty = sim->bulk_dirty = false;
   return SWIM_OK;
 }
 
@@ -572,17 +576,22 @@ __global__ void __launch_bounds__(kGT) add_members_kernel(SimDev d, uint32_t rou
   if (lane == 0 && (added || full)) { atomicAdd(&res[0], (u64)added); atomicAdd(&res[1], (u64)full); }
 }
 
-// after a bulk edit: the rows changed on the device; the mail graph is rebuilt by the next step, the last round's
-// envelopes no longer match the rows and the checkpoint belongs to the old view
+// after a bulk edit: the rows changed on the device; the mail graph is rebuilt by the next step (on a sharded handle by
+// every rank together), the last round's envelopes no longer match the rows and the checkpoint belongs to the old view
 void mark_edited(swim_sim *sim) {
-  sim->edges_dirty = true;
+  sim->bulk_dirty = true;
   sim->tdead_dirty = true;
   sim->rows_edited = true;
   sim->ckpt_valid = false;
 }
 
+// A sharded handle changes memberships together with its peers (the next step rebuilds the mail graph as a collective):
+// it must be connected to them first.
 int edit_preamble(swim_sim *sim, const char *api) {
-  if (sim->dev.world != 1) { set_error(sim, "%s: view membership changes are single-shard only", api); return SWIM_ESTATE; }
+  if (sim->dev.world != 1 && !sim->connected) {
+    set_error(sim, "%s: world > 1 needs swim_sim_ipc_connect or swim_sim_connect (every rank makes the same call)", api);
+    return SWIM_ESTATE;
+  }
   cudaSetDevice(sim->device);
   return SWIM_OK;
 }
@@ -591,14 +600,41 @@ int row_grid(const swim_sim *sim, size_t rows) { return grid_of(sim, (rows + kGW
 
 } // namespace
 
-// Rebuild the mail graph from the device rows (after membership changes), in place: no host copy.
+// Rebuild the mail graph from the device rows (after membership changes), in place: no host copy. Sharded: a collective
+// of the first step after a bulk call — barrier, every rank's rows gathered into one global matrix, the existing sharded
+// build, and (over peer memory) the peers' new mail-flag arrays mapped before the old ones are freed.
 namespace swim {
 int rebuild_edges_from_device(swim_sim *sim) {
   SimDev &d = sim->dev;
-  if (d.world != 1) { set_error(sim, "view membership changes are single-shard only"); return SWIM_ESTATE; }
-  int rc = build_graph(sim, d.nbr, nullptr);
-  if (rc) return rc;
-  sim->edges_dirty = false;
+  if (d.world == 1) {
+    int rc = build_graph(sim, d.nbr, nullptr);
+    if (rc) return rc;
+    sim->edges_dirty = sim->bulk_dirty = false;
+    return SWIM_OK;
+  }
+  if (sim->edges_dirty) { // only this rank made the change: its peers would never join the rebuild
+    set_error(sim, "a scalar membership change on a sharded handle (view changes of a sharded run go through "
+                   "swim_sim_remove_dead_nodes / swim_sim_add_members / swim_sim_push_pull on every rank)");
+    return SWIM_ESTATE;
+  }
+  if (sim->failed) { set_error(sim, "swim_sim_step: an earlier call failed part-way; the handle's device state is undefined"); return SWIM_ESTATE; }
+  uint8_t *retired = nullptr;
+  const int rc = [&]() -> int {
+    int r;
+    if ((r = coll_barrier(sim))) return r; // every rank's edits are done
+    {
+      Scratch s(sim);
+      uint32_t *g;
+      SCRATCH(s, g, (size_t)d.world * d.per * d.cap);
+      if ((r = coll_gather(sim, kCollNbr, g))) return r;
+      if ((r = build_graph(sim, g, nullptr, d.p2p ? &retired : nullptr))) return r;
+    } // (scratch freed here: every free of the call comes before its last barrier)
+    if (d.p2p) { uint8_t *x = retired; retired = nullptr; return coll_remap_eflag(sim, x); }
+    return coll_barrier(sim);
+  }();
+  if (retired) cudaFree(retired);
+  if (rc) { sim->failed = true; return rc; } // the ranks are no longer in step
+  sim->bulk_dirty = false;
   return SWIM_OK;
 }
 } // namespace swim
@@ -662,28 +698,31 @@ extern "C" int swim_sim_add_members(swim_sim_t *sim, const swim_member_add_t *ad
       return SWIM_EINVAL;
     }
   u64 h[2] = {0, 0};
-  if (n) {
+  // sharded: every rank is given the same list and applies the adds of its own observers
+  std::vector<uint32_t> order;
+  for (size_t x = 0; x < n; ++x)
+    if (adds[x].observer - d.first < d.n) order.push_back((uint32_t)x);
+  const size_t nl = order.size();
+  if (nl) {
     // one group per observer, its adds in the order given
-    std::vector<uint32_t> order(n);
-    for (size_t x = 0; x < n; ++x) order[x] = (uint32_t)x;
     std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return adds[a].observer < adds[b].observer; });
-    std::vector<uint4> sorted(n);
+    std::vector<uint4> sorted(nl);
     std::vector<uint32_t> grp;
-    for (size_t x = 0; x < n; ++x) {
+    for (size_t x = 0; x < nl; ++x) {
       const swim_member_add_t &a = adds[order[x]];
       sorted[x] = make_uint4(a.observer, a.member, a.incarnation, 0u);
       if (x == 0 || a.observer != adds[order[x - 1]].observer) grp.push_back((uint32_t)x);
     }
     const uint32_t ngroups = (uint32_t)grp.size();
-    grp.push_back((uint32_t)n);
+    grp.push_back((uint32_t)nl);
     Scratch s(sim);
     uint4 *d_adds;
     uint32_t *d_grp;
     u64 *res;
-    SCRATCH(s, d_adds, n);
+    SCRATCH(s, d_adds, nl);
     SCRATCH(s, d_grp, grp.size());
     SCRATCH(s, res, 2);
-    GRAPH_TRY(sim, cudaMemcpyAsync(d_adds, sorted.data(), n * sizeof(uint4), cudaMemcpyHostToDevice, sim->stream));
+    GRAPH_TRY(sim, cudaMemcpyAsync(d_adds, sorted.data(), nl * sizeof(uint4), cudaMemcpyHostToDevice, sim->stream));
     GRAPH_TRY(sim, cudaMemcpyAsync(d_grp, grp.data(), grp.size() * 4, cudaMemcpyHostToDevice, sim->stream));
     GRAPH_TRY(sim, cudaMemsetAsync(res, 0, 16, sim->stream));
     const int g = row_grid(sim, ngroups);
@@ -699,9 +738,10 @@ extern "C" int swim_sim_add_members(swim_sim_t *sim, const swim_member_add_t *ad
     ++sim->launches;
     GRAPH_TRY(sim, cudaMemcpyAsync(h, res, sizeof h, cudaMemcpyDeviceToHost, sim->stream));
     GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
-    mark_edited(sim);
-    if (h[0]) sim->view_set = true;
   }
+  // (sharded: every rank saw the same list, so all of them mark the view changed and rebuild together)
+  if (n) mark_edited(sim);
+  if (h[0] || (d.world > 1 && n)) sim->view_set = true;
   if (n_added) *n_added = h[0];
   if (n_full) *n_full = h[1];
   return SWIM_OK;

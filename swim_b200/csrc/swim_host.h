@@ -8,6 +8,27 @@
 
 #include "swim_device.cuh"
 
+namespace swim {
+// Device block of one rank for the collectives between steps (swim_dist.cu): the barrier words its peers store into, the
+// values they bring to a barrier, and this rank's current mail-flag array for the peers to map after a sharded rebuild.
+struct CollBlock {
+  uint32_t bar[SWIM_MAX_WORLD];                 // bar[q] = the last barrier generation peer q reached
+  unsigned long long val[2][SWIM_MAX_WORLD];    // [generation parity][q] the value peer q brought to that barrier
+  unsigned long long got[SWIM_MAX_WORLD];       // the peers' values of the last barrier, for the host
+  uint32_t seen[SWIM_MAX_WORLD];                // bar[] as the last poll of the host's barrier wait read it
+  cudaIpcMemHandle_t eflag_h;                   // eflag: handle, raw pointer (ranks of one process) and parity stride
+  unsigned long long eflag_raw;
+  uint32_t estride, _pad;
+};
+// The peers' arrays the collectives read (mapped by swim_sim_ipc_connect; entry [rank] is unused).
+struct PeerViews {
+  CollBlock *coll[SWIM_MAX_WORLD];
+  const uint32_t *nbr[SWIM_MAX_WORLD], *vinc[SWIM_MAX_WORLD], *self_inc[SWIM_MAX_WORLD];
+  const uint8_t *vst[SWIM_MAX_WORLD];
+  bool same_process[SWIM_MAX_WORLD];
+};
+} // namespace swim
+
 struct swim_sim {
   swim_config_t cfg{};
   swim::SimDev dev{};
@@ -19,7 +40,10 @@ struct swim_sim {
   bool timed = false;
   uint32_t round = 0;
   bool view_set = false;
-  bool edges_dirty = false; // scalar or bulk calls changed a row's membership: the mail graph is rebuilt by the next step
+  bool edges_dirty = false; // a scalar call changed a row's membership: the mail graph is rebuilt by the next step (one
+                            //   shard only: a sharded handle refuses that step, its peers would not join the rebuild)
+  bool bulk_dirty = false;  // a bulk call (remove_dead_nodes, add_members, push_pull with inserts) changed memberships: the
+                            //   next step rebuilds the mail graph — on a sharded handle together with every peer
   bool rows_edited = false; // a bulk membership edit since the last step: the last round's envelopes no longer match the rows
   bool tdead_dirty = true;  // crashed-member bitmaps must be rebuilt from alive[]
   bool connected = false;   // multi-shard exchange ready
@@ -67,6 +91,9 @@ struct swim_sim {
   uint32_t churn_last_round = 0xFFFFFFF0u; // last round churn_kernel ran for (its list counter has round-parity slots)
   std::vector<void *> ipc_opened; // peer mappings to close
   void *dist = nullptr; // multi-GPU exchange state (swim_dist.cu)
+  swim::CollBlock *d_coll = nullptr; // this rank's block of the collectives between steps
+  uint32_t coll_gen = 0;             // barriers run so far (every rank runs the same sequence)
+  swim::PeerViews peer{};
 };
 
 namespace swim {
@@ -80,4 +107,9 @@ int prof_begin(swim_sim *sim, int phase);
 void prof_end(swim_sim *sim, int mark);
 int prof_collect(swim_sim *sim);
 void dist_teardown(swim_sim *sim);
+// Collectives between steps of a connected sharded handle (swim_dist.cu): every rank calls them in the same order.
+int coll_barrier(swim_sim *sim, unsigned long long mine = 0, unsigned long long *sum = nullptr);
+enum CollArray { kCollNbr, kCollVst, kCollVinc, kCollSelfInc };
+int coll_gather(swim_sim *sim, CollArray which, void *out);
+int coll_remap_eflag(swim_sim *sim, uint8_t *retired);
 } // namespace swim

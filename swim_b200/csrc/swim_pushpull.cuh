@@ -6,45 +6,56 @@
 // the two swap their full member state. Each side merges what it receives through the receive path's state machine
 // (row_apply), and a merge inserts the Alive members it did not list — the only way a bulk run learns unknown members.
 // Everything that is sent is read from a snapshot taken before any row changes, so the result does not depend on the
-// order in which warps run.
+// order in which warps run. On a sharded handle the call is a collective: the snapshot is every rank's rows gathered
+// into global-id order, every rank draws the partners of all N nodes from it (the draws are a function of the snapshot,
+// alive[] and the round, so all ranks agree without exchanging them), and each rank merges into its own receivers.
 #pragma once
 
 #include "swim_graph.cuh"
 
 namespace {
 
-// One thread per node: the partner p_i = the floor(x L / 2^32)-th Alive slot (ascending), x = word 0 of Philox block
-// (round, i, P_PUSHPULL, 0). part[i] = p_i if i and p_i are both up, else SWIM_NO_MEMBER; cnt[p_i] counts p_i's choosers.
-__global__ void __launch_bounds__(kGT) pp_pick_kernel(SimDev d, uint32_t round, uint32_t *part, uint32_t *cnt, u64 *n_ex) {
+// One thread per node i of rows [0, rows) of (nbr, vst), which start at global id 0: this shard's own rows on a single
+// shard, the gathered global snapshot on several. The partner p_i = the floor(x L / 2^32)-th Alive slot (ascending),
+// x = word 0 of Philox block (round, i, P_PUSHPULL, 0); p_i = SWIM_NO_MEMBER unless i and p_i are both up. For the
+// local nodes i: part[i - first] = p_i. For the local partners p_i: cnt[p_i - first] counts p_i's choosers, and
+// key[i] = p_i (SWIM_NO_MEMBER otherwise; key = null on a single shard, where part is that array).
+__global__ void __launch_bounds__(kGT) pp_pick_kernel(SimDev d, uint32_t round, const uint32_t *nbr, const uint8_t *vst,
+                                                      uint32_t rows, uint32_t *part, uint32_t *key, uint32_t *cnt, u64 *n_ex) {
   uint32_t ex = 0;
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < d.n; i += gridDim.x * blockDim.x) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < rows; i += gridDim.x * blockDim.x) {
     uint32_t p = SWIM_NO_MEMBER;
     if (d.alive[i]) {
-      const uint8_t *st = d.vst + (size_t)i * d.cap;
+      const uint8_t *st = vst + (size_t)i * d.cap;
       uint32_t L = 0;
       for (uint32_t s = 0; s < d.cap; ++s) L += (st[s] & 3u) == SWIM_ALIVE;
       if (L) {
         uint32_t k = bounded(philox4x32_10(make_uint4(round, i, P_PUSHPULL, 0), d.key0, d.key1).x, L), s = 0;
         for (;; ++s)
           if ((st[s] & 3u) == SWIM_ALIVE && k-- == 0) break;
-        p = d.nbr[(size_t)i * d.cap + s];
-        if (d.alive[p]) { atomicAdd(&cnt[p], 1u); ++ex; }
-        else p = SWIM_NO_MEMBER;
+        p = nbr[(size_t)i * d.cap + s];
+        if (!d.alive[p]) p = SWIM_NO_MEMBER;
       }
     }
-    part[i] = p;
+    const bool to_me = p != SWIM_NO_MEMBER && p - d.first < d.n;
+    if (to_me) atomicAdd(&cnt[p - d.first], 1u);
+    if (i - d.first < d.n) {
+      part[i - d.first] = p;
+      ex += p != SWIM_NO_MEMBER;
+    }
+    if (key) key[i] = to_me ? p : SWIM_NO_MEMBER;
   }
   ex = __reduce_add_sync(kFull, ex);
   if ((threadIdx.x & 31) == 0 && ex) atomicAdd(n_ex, (u64)ex);
 }
 
-// The sender's state as the snapshot holds it.
+// The senders' state as the snapshot holds it, by global id.
 struct PpSnap {
   const uint32_t *nbr, *vinc, *self_inc;
   const uint8_t *vst;
 };
 
-// One warp per receiver j: senders {part[j]} ∪ choosers(j) in ascending id, each once; record by record through
+// One warp per local receiver j (global id first + j): senders {part[j]} ∪ choosers(j) in ascending id, each once; record by record through
 // row_apply (net), insertion of unknown Alive members, re-broadcast of every `Just`. res = {inserted, dropped on a full row}.
 template <int W>
 __global__ void __launch_bounds__(kThreads) push_pull_kernel(SimDev d, uint32_t round, PpSnap snap, const uint32_t *part,
@@ -105,7 +116,7 @@ __global__ void __launch_bounds__(kThreads) push_pull_kernel(SimDev d, uint32_t 
                          lv == SWIM_ALIVE ? SWIM_MSG_ALIVE : lv == SWIM_SUSPECT ? SWIM_MSG_SUSPECT : SWIM_MSG_DEAD);
         }
         uint4 rb;
-        const int v = row_apply<W>(row, d, j, self_inc, rec, rb, lane, c.v[SWIM_CTR_REFUTES]);
+        const int v = row_apply<W>(row, d, d.first + j, self_inc, rec, rb, lane, c.v[SWIM_CTR_REFUTES]);
         if (v == 2) { // an Alive member j does not list: addNewMember (Core.hs:206-216), as swim_alive_node inserts
           if (used == d.cap) { ++full; continue; }
           uint32_t pos = 0;
@@ -146,46 +157,53 @@ __global__ void __launch_bounds__(kThreads) push_pull_kernel(SimDev d, uint32_t 
 
 } // namespace
 
-extern "C" int swim_sim_push_pull(swim_sim_t *sim, uint64_t *n_exchanges, uint64_t *n_inserted, uint64_t *n_full) {
-  if (!sim) return SWIM_EINVAL;
+namespace {
+// The exchange on this shard's receivers. Sharded: between the gather barriers of swim_sim_push_pull, with `snap` the
+// gathered global snapshot. h = {inserted, dropped on a full row, exchanges} of this shard.
+int push_pull_local(swim_sim *sim, Scratch &s, const PpSnap *gsnap, u64 h[3]) {
   const SimDev &d = sim->dev;
-  if (d.world != 1) { set_error(sim, "swim_sim_push_pull: single shard only (a partner's row may live on another rank)"); return SWIM_ESTATE; }
-  if (!sim->view_set) { set_error(sim, "swim_sim_push_pull: no view installed"); return SWIM_ESTATE; }
-  if (sim->failed) { set_error(sim, "swim_sim_push_pull: an earlier step failed part-way; the handle's device state is undefined"); return SWIM_ESTATE; }
-  cudaSetDevice(sim->device);
   const size_t n = d.n, slots = n * d.cap;
-  Scratch s(sim);
-  uint32_t *part, *cnt;
-  u64 *seg, *res, h[3] = {0, 0, 0}, E = 0;
+  const uint32_t rows = gsnap ? d.N : d.n; // the rows the partners are drawn from
+  uint32_t *part, *cnt, *key = nullptr;
+  u64 *seg, *res, E = 0, ex = 0;
   SCRATCH(s, part, n);
   SCRATCH(s, cnt, n);
   SCRATCH(s, seg, n + 1);
   SCRATCH(s, res, 3);
+  if (gsnap) SCRATCH(s, key, rows);
   GRAPH_TRY(sim, cudaMemsetAsync(cnt, 0, n * 4, sim->stream));
   GRAPH_TRY(sim, cudaMemsetAsync(res, 0, 3 * 8, sim->stream));
-  SWIM_LAUNCH(pp_pick_kernel, grid_of(sim, (n + kGT - 1) / kGT), kGT, sim->stream, d, sim->round, part, cnt, res + 2);
+  const uint32_t *pn = gsnap ? gsnap->nbr : d.nbr;
+  const uint8_t *pv = gsnap ? gsnap->vst : d.vst;
+  SWIM_LAUNCH(pp_pick_kernel, grid_of(sim, (rows + kGT - 1) / kGT), kGT, sim->stream, d, sim->round, pn, pv, rows, part, key,
+              cnt, res + 2);
   ++sim->launches;
   GRAPH_TRY(sim, cudaGetLastError());
   int rc;
   if ((rc = scan_u32(sim, s, cnt, n, seg))) return rc;
   GRAPH_TRY(sim, cudaMemcpyAsync(&E, seg + n, 8, cudaMemcpyDeviceToHost, sim->stream));
+  GRAPH_TRY(sim, cudaMemcpyAsync(&ex, res + 2, 8, cudaMemcpyDeviceToHost, sim->stream));
   GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
-  if (E) {
-    // the choosers of every node, ascending: a stable sort of the partner array by partner
-    const uint32_t *key, *chooser;
-    if ((rc = sort_by_key(sim, s, part, n, 1, E, d.N, &key, &chooser))) return rc;
+  if (E || ex) { // (sharded, a shard's nodes may pull from partners elsewhere while none of its own is chosen)
+    // the choosers of every local node, ascending: a stable sort of the partner array by partner
+    const uint32_t *skey, *chooser = nullptr;
+    if (E && (rc = sort_by_key(sim, s, key ? key : part, rows, 1, E, d.N, &skey, &chooser))) return rc;
     PpSnap snap;
-    uint32_t *nb, *vi, *si;
-    uint8_t *vs;
-    SCRATCH(s, nb, slots);
-    SCRATCH(s, vi, slots);
-    SCRATCH(s, si, n);
-    SCRATCH(s, vs, slots);
-    GRAPH_TRY(sim, cudaMemcpyAsync(nb, d.nbr, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
-    GRAPH_TRY(sim, cudaMemcpyAsync(vi, d.vinc, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
-    GRAPH_TRY(sim, cudaMemcpyAsync(si, d.self_inc, n * 4, cudaMemcpyDeviceToDevice, sim->stream));
-    GRAPH_TRY(sim, cudaMemcpyAsync(vs, d.vst, slots, cudaMemcpyDeviceToDevice, sim->stream));
-    snap.nbr = nb; snap.vinc = vi; snap.self_inc = si; snap.vst = vs;
+    if (gsnap) {
+      snap = *gsnap;
+    } else {
+      uint32_t *nb, *vi, *si;
+      uint8_t *vs;
+      SCRATCH(s, nb, slots);
+      SCRATCH(s, vi, slots);
+      SCRATCH(s, si, n);
+      SCRATCH(s, vs, slots);
+      GRAPH_TRY(sim, cudaMemcpyAsync(nb, d.nbr, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
+      GRAPH_TRY(sim, cudaMemcpyAsync(vi, d.vinc, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
+      GRAPH_TRY(sim, cudaMemcpyAsync(si, d.self_inc, n * 4, cudaMemcpyDeviceToDevice, sim->stream));
+      GRAPH_TRY(sim, cudaMemcpyAsync(vs, d.vst, slots, cudaMemcpyDeviceToDevice, sim->stream));
+      snap.nbr = nb; snap.vinc = vi; snap.self_inc = si; snap.vst = vs;
+    }
     const int g = grid_of(sim, (n + kWarpsPerBlock - 1) / kWarpsPerBlock);
     const uint32_t *cp = part;
     const u64 *cs = seg;
@@ -198,9 +216,62 @@ extern "C" int swim_sim_push_pull(swim_sim_t *sim, uint64_t *n_exchanges, uint64
     ++sim->launches;
     GRAPH_TRY(sim, cudaGetLastError());
   }
-  GRAPH_TRY(sim, cudaMemcpyAsync(h, res, sizeof h, cudaMemcpyDeviceToHost, sim->stream));
+  GRAPH_TRY(sim, cudaMemcpyAsync(h, res, 3 * sizeof(u64), cudaMemcpyDeviceToHost, sim->stream));
   GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
-  if (h[0]) mark_edited(sim); // members were inserted: the mail graph is rebuilt by the next step
+  return SWIM_OK;
+}
+
+// Sharded: barrier (every rank's earlier calls are done), gather the global snapshot, barrier (nobody changes a row
+// before every rank has its copy), the local exchange, and a last barrier that sums the inserts, so that every rank
+// marks the view changed — and rebuilds at the next step — exactly when some rank inserted. The scratch is freed before
+// that barrier: a peer that shares this device may start its round kernels right after it, and cudaFree would wait for
+// them while they wait for this rank.
+int push_pull_sharded(swim_sim *sim, u64 h[3], u64 *inserted_all) {
+  const SimDev &d = sim->dev;
+  const size_t rows = (size_t)d.world * d.per, gslots = rows * d.cap;
+  int rc;
+  {
+    Scratch s(sim);
+    uint32_t *nb, *vi, *si;
+    uint8_t *vs;
+    SCRATCH(s, nb, gslots);
+    SCRATCH(s, vi, gslots);
+    SCRATCH(s, si, rows);
+    SCRATCH(s, vs, gslots);
+    if ((rc = coll_barrier(sim))) return rc;
+    if ((rc = coll_gather(sim, kCollNbr, nb)) || (rc = coll_gather(sim, kCollVst, vs)) ||
+        (rc = coll_gather(sim, kCollVinc, vi)) || (rc = coll_gather(sim, kCollSelfInc, si)))
+      return rc;
+    if ((rc = coll_barrier(sim))) return rc;
+    PpSnap snap;
+    snap.nbr = nb; snap.vinc = vi; snap.self_inc = si; snap.vst = vs;
+    if ((rc = push_pull_local(sim, s, &snap, h))) return rc;
+  }
+  return coll_barrier(sim, h[0], inserted_all);
+}
+} // namespace
+
+extern "C" int swim_sim_push_pull(swim_sim_t *sim, uint64_t *n_exchanges, uint64_t *n_inserted, uint64_t *n_full) {
+  if (!sim) return SWIM_EINVAL;
+  const SimDev &d = sim->dev;
+  if (d.world != 1 && !sim->connected) {
+    set_error(sim, "swim_sim_push_pull: world > 1 needs swim_sim_ipc_connect or swim_sim_connect (every rank makes the call)");
+    return SWIM_ESTATE;
+  }
+  if (!sim->view_set) { set_error(sim, "swim_sim_push_pull: no view installed"); return SWIM_ESTATE; }
+  if (sim->failed) { set_error(sim, "swim_sim_push_pull: an earlier step failed part-way; the handle's device state is undefined"); return SWIM_ESTATE; }
+  cudaSetDevice(sim->device);
+  u64 h[3] = {0, 0, 0}, ins = 0;
+  if (d.world == 1) {
+    Scratch s(sim);
+    int rc = push_pull_local(sim, s, nullptr, h);
+    if (rc) return rc;
+    ins = h[0];
+  } else {
+    int rc = push_pull_sharded(sim, h, &ins);
+    if (rc) { sim->failed = true; return rc; } // the ranks are no longer in step
+  }
+  if (ins) mark_edited(sim); // members were inserted: the mail graph is rebuilt by the next step
   else sim->tdead_dirty = true;
   if (n_exchanges) *n_exchanges = h[2];
   if (n_inserted) *n_inserted = h[0];

@@ -254,6 +254,7 @@ extern "C" int swim_sim_create(const swim_config_t *cfg, swim_sim_t **out) {
     if ((r = dalloc(sim, &sim->d_obs_done, 2, 0))) return r;
     if ((r = dalloc(sim, &d.gbar, 4, 0))) return r;
     if ((r = dalloc(sim, &d.qm, 4, 0))) return r;
+    if ((r = dalloc(sim, &sim->d_coll, 1, 0))) return r; // barrier words of the collectives between steps
     return SWIM_OK;
   }();
   if (rc) { g_last_error = sim->last_error; swim_sim_destroy(sim); return rc; }
@@ -558,7 +559,7 @@ static int step_async_impl(swim_sim_t *sim, uint32_t rounds, bool timed) {
   if (!sim) return SWIM_EINVAL;
   if (!sim->view_set) { set_error(sim, "swim_sim_step: no view installed (swim_sim_set_view / swim_set_members)"); return SWIM_ESTATE; }
   cudaSetDevice(sim->device);
-  if (sim->edges_dirty) {
+  if (sim->edges_dirty || sim->bulk_dirty) {
     int rc = swim::rebuild_edges_from_device(sim);
     if (rc) return rc;
   }
@@ -690,7 +691,7 @@ static void ckpt_sources(const swim_sim *sim, std::vector<std::pair<void *, size
 
 extern "C" int swim_sim_save(swim_sim_t *sim) {
   if (!sim) return SWIM_EINVAL;
-  if (!sim->view_set || sim->edges_dirty) { set_error(sim, "swim_sim_save: no view installed, or memberships changed since the last step"); return SWIM_ESTATE; }
+  if (!sim->view_set || sim->edges_dirty || sim->bulk_dirty) { set_error(sim, "swim_sim_save: no view installed, or memberships changed since the last step"); return SWIM_ESTATE; }
   cudaSetDevice(sim->device);
   const SimDev &d = sim->dev;
   if (sim->tdead_dirty) { // the saved per-node records are current
@@ -718,7 +719,7 @@ extern "C" int swim_sim_save(swim_sim_t *sim) {
 
 extern "C" int swim_sim_load(swim_sim_t *sim) {
   if (!sim) return SWIM_EINVAL;
-  if (!sim->ckpt_valid || sim->edges_dirty || sim->ckpt_epoch != sim->view_epoch) {
+  if (!sim->ckpt_valid || sim->edges_dirty || sim->bulk_dirty || sim->ckpt_epoch != sim->view_epoch) {
     set_error(sim, "swim_sim_load: no checkpoint of this view (swim_sim_save first; a new view or a membership change drops it)");
     return SWIM_ESTATE;
   }

@@ -136,14 +136,16 @@ class Simulator:
 
     def remove_dead_nodes(self, min_age=0):
         """removeDeadNodes (Core.hs:65-67) on every local store: Dead entries at least `min_age` rounds old leave.
-        Returns the number removed. Single shard; the next step rebuilds the mail graph."""
+        Returns the number removed on this shard; the next step rebuilds the mail graph. On a sharded handle a
+        collective: every rank makes the call (the rebuild in the next step is done by all ranks together)."""
         n = C.c_uint64()
         check(lib().swim_sim_remove_dead_nodes(self._h, min_age, C.byref(n)), "swim_sim_remove_dead_nodes", self._h)
         return n.value
 
     def add_members(self, observers, members, incarnations=0):
         """addNewMember (Core.hs:206-216) for many stores, in the order given: an unlisted member is inserted Alive with
-        its incarnation, a listed one is left alone, an add to a full row is dropped. Returns (added, full)."""
+        its incarnation, a listed one is left alone, an add to a full row is dropped. Returns (added, full) of this shard.
+        On a sharded handle a collective: every rank is given the same global list and applies its own observers' adds."""
         observers = np.atleast_1d(np.asarray(observers))
         adds = np.zeros(len(observers), dtype=A.MEMBER_ADD_DTYPE)
         adds["observer"] = observers
@@ -157,7 +159,8 @@ class Simulator:
     def push_pull(self):
         """Push-pull state exchange (DESIGN.md 2.6) at the current round: every up node swaps its full member state with
         one random Alive member, and each side merges what it receives, inserting the Alive members it did not list.
-        Single shard. Returns (exchanges, inserted, full)."""
+        Returns (exchanges, inserted, full) of this shard. On a sharded handle a collective: every rank makes the call,
+        each on its own host thread or process."""
         e, n, f = C.c_uint64(), C.c_uint64(), C.c_uint64()
         check(lib().swim_sim_push_pull(self._h, C.byref(e), C.byref(n), C.byref(f)), "swim_sim_push_pull", self._h)
         return e.value, n.value, f.value

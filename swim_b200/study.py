@@ -97,8 +97,8 @@ def latency_stats(hist):
 def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None, push_pull_every=0):
     """Step `rounds` rounds, sampling the convergence count; returns the time series, the final counters and the final
     view report. `reduce_sum(list_of_numbers) -> list` adds values over ranks (identity for one GPU). push_pull_every = R
-    > 0: a push-pull state exchange (Simulator.push_pull, single shard) after every R-th round; its summed outputs are
-    in "push_pull"."""
+    > 0: a push-pull state exchange (Simulator.push_pull; on a sharded handle a collective, which every rank reaches at
+    the same round) after every R-th round; its outputs, summed over the calls and the ranks, are in "push_pull"."""
     red = reduce_sum or (lambda xs: xs)
     series = []
     done = 0
@@ -126,5 +126,5 @@ def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None, push_
     out = {"mismatch_series": series, "counters": dict(zip(A.CTR_NAMES, counters)), "report": rep,
            "device_ms": device_ms, "device_us_per_round": device_ms * 1e3 / max(1, rounds)}
     if push_pull_every:
-        out["push_pull"] = dict(zip(("exchanges", "inserted", "full"), pp))
+        out["push_pull"] = dict(zip(("exchanges", "inserted", "full"), (int(v) for v in red(pp))))
     return out
