@@ -146,6 +146,8 @@ foreign import ccall safe   "swim_sim_remove_dead_nodes" c_simRemoveDeadNodes ::
 foreign import ccall safe   "swim_sim_add_members"     c_simAddMembers     :: Sim -> Ptr Word32 -> CSize -> Ptr Word64 -> Ptr Word64 -> IO CInt
 -- push-pull anti-entropy between steps (memberlist; joinHosts, Types.hs:47, completed): exchanges, inserted, full
 foreign import ccall safe   "swim_sim_push_pull"       c_simPushPull       :: Sim -> Ptr Word64 -> Ptr Word64 -> Ptr Word64 -> IO CInt
+-- the view graph generated on the device (kind = SWIM_TOPO_*, degree, seed) and installed as by swim_sim_set_view_device
+foreign import ccall safe   "swim_sim_generate_view"   c_simGenerateView   :: Sim -> CInt -> Word32 -> Word64 -> IO CInt
 foreign import ccall unsafe "swim_envelope_encode"     c_envEncode         :: Ptr () -> CSize -> Ptr Word8 -> CSize -> Ptr CSize -> IO CInt
 foreign import ccall unsafe "swim_envelope_decode"     c_envDecode         :: Ptr Word8 -> CSize -> Ptr () -> CSize -> Ptr CSize -> IO CInt
 

@@ -256,10 +256,20 @@ int swim_sim_set_view_device(swim_sim_t *sim, const uint32_t *nbr_global_dev);
 
 /* Host-side synthetic topologies (BASELINE configs): rows of `degree` distinct ids != i.
  * kind 0 = complete (degree ignored, needs N-1 <= view_cap), 1 = uniform random,
- * 2 = ring lattice (i±1..±degree/2). out is [N*view_cap]. No device needed. */
-enum { SWIM_TOPO_COMPLETE = 0, SWIM_TOPO_RANDOM = 1, SWIM_TOPO_RING = 2 };
+ * 2 = ring lattice (i±1..±degree/2), 3 = symmetric random: the union of degree/2 random
+ * Hamiltonian cycles (DESIGN.md §2.3, purpose 11), j in row i exactly when i is in row j,
+ * between 2 and degree members per row (fewer than degree where cycles repeat a neighbour);
+ * degree must be even and N >= 3 (SWIM_EINVAL otherwise). out is [N*view_cap]. No device needed. */
+enum { SWIM_TOPO_COMPLETE = 0, SWIM_TOPO_RANDOM = 1, SWIM_TOPO_RING = 2, SWIM_TOPO_SYMMETRIC = 3 };
 int swim_topology_generate(int kind, uint32_t n_nodes, uint32_t view_cap, uint32_t degree,
                            uint64_t seed, uint32_t *out_nbr);
+
+/* The same matrix generated on the device, in temporary device memory on the handle's stream, and installed as
+ * swim_sim_set_view_device installs it (same checks, SWIM_ESTATE after swim_sim_ipc_connect, the checkpoint dropped).
+ * Bit-identical to swim_topology_generate(kind, N, view_cap, degree, seed, .) for every kind. On a sharded handle every
+ * rank generates the whole global matrix itself (no communication). The temporary memory is freed before the call
+ * returns. */
+int swim_sim_generate_view(swim_sim_t *sim, int kind, uint32_t degree, uint64_t seed);
 
 /* ====================== bulk path: the accelerated protocol loop =====================
  * Replaces the ticker + the three conduits of Core.main (Core.hs:233-241, 279-287). */

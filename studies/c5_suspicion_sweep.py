@@ -34,7 +34,9 @@ def main():
     ap.add_argument("--crash-ppm", type=int, default=1000)
     ap.add_argument("--loss-ppm", type=int, default=0)
     ap.add_argument("--flags", type=int, default=0, help="SWIM_F_* protocol variants")
-    ap.add_argument("--topology", default="random", choices=["random", "ring"])
+    ap.add_argument("--topology", default="random", choices=["random", "ring", "symmetric"],
+                    help="view graph, generated on the device: directed random views, a ring lattice, or symmetric random "
+                         "views (j lists i exactly when i lists j)")
     ap.add_argument("--sample-every", type=int, default=10)
     ap.add_argument("--push-pull-every", type=int, default=0, metavar="R",
                     help="a push-pull state exchange (memberlist anti-entropy) after every R-th round (a collective "
@@ -44,7 +46,7 @@ def main():
 
     import torch
     from swim_b200 import dist as sd
-    from swim_b200.sim import Simulator, default_config, generate_topology
+    from swim_b200.sim import Simulator, default_config
     from swim_b200.study import run_sweep_point
 
     rank, world, local = sd.init_from_env()
@@ -52,9 +54,6 @@ def main():
         raise SystemExit("c5_suspicion_sweep needs a CUDA device (there is no CPU fallback)")
     torch.cuda.set_device(local)
     n = args.nodes_per_gpu * world
-    t0 = time.perf_counter()
-    nbr = generate_topology(args.topology, n, 32, 32, seed=args.seed & 0xFFFF)
-    t_topo = time.perf_counter() - t0
     red = (lambda xs: [int(v) for v in sd.global_sum(xs)]) if world > 1 else None
 
     def barrier():
@@ -68,11 +67,12 @@ def main():
                          world=world, device=local, flags=args.flags, churn_ppm=args.crash_ppm, rejoin_min=10, rejoin_max=50)
     t0 = time.perf_counter()
     sim = Simulator(cfg)
-    sim.set_view(nbr)
+    t1 = time.perf_counter()
+    sim.generate_view(args.topology, 32, seed=args.seed & 0xFFFF)  # every rank generates the global matrix on its GPU
+    t_topo = time.perf_counter() - t1
     mode = sd.connect(sim)
-    del nbr
     sim.save()
-    t_setup = time.perf_counter() - t0
+    t_setup = time.perf_counter() - t0 - t_topo
     for S in args.suspicion:
         barrier()
         sim.load()
@@ -95,7 +95,7 @@ def main():
                     "device_us_per_round_rank0": res["device_us_per_round"],
                     "node_rounds_per_s_device_rank0": n * args.rounds / max(1e-9, res["device_ms"] * 1e-3),
                     "node_rounds_per_s_wall": n * args.rounds / wall,
-                    "setup_s": {"topology": t_topo, "create_set_view_connect_save": t_setup}}
+                    "setup_s": {"topology": t_topo, "create_connect_save": t_setup}}
             if args.push_pull_every:
                 line["config"]["push_pull_every"] = args.push_pull_every
                 line["push_pull"] = res["push_pull"]

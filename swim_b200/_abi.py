@@ -20,7 +20,7 @@ IPC_BLOB_BYTES = 1024
 
 EV_CRASH, EV_REJOIN, EV_INJECT = 0, 1, 2
 F_NONE, F_STRICT_OVERRIDE, F_ROUND_ROBIN = 0, 1, 2  # SWIM_F_*: protocol variants
-TOPO_COMPLETE, TOPO_RANDOM, TOPO_RING = 0, 1, 2
+TOPO_COMPLETE, TOPO_RANDOM, TOPO_RING, TOPO_SYMMETRIC = 0, 1, 2, 3
 
 (ARR_ALIVE, ARR_SELF_INC, ARR_SEQNO, ARR_NBR, ARR_VST, ARR_VINC, ARR_VLAST, ARR_PB, ARR_PB_CNT, ARR_BACK_AT,
  ARR_LAST_CRASH, ARR_LAST_REJOIN) = range(12)

@@ -49,6 +49,7 @@ def lib():
     sig("swim_sim_add_members", i, vp, vp, sz, P(u64), P(u64))
     sig("swim_sim_push_pull", i, vp, P(u64), P(u64), P(u64))
     sig("swim_topology_generate", i, i, u32, u32, u32, u64, vp)
+    sig("swim_sim_generate_view", i, vp, i, u32, u64)
     sig("swim_sim_set_round", i, vp, u32)
     sig("swim_sim_save", i, vp)
     sig("swim_sim_set_params", i, vp, P(A.Config))

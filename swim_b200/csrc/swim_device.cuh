@@ -64,7 +64,7 @@ constexpr long long kPeerWaitCycles = 120000000000ll; // ~60 s at 2 GHz, then th
 // Philox counter purposes (DESIGN.md §2.3). TARGET and LOSS0 blocks are shared by the four nodes
 // 4g..4g+3 (counter word 1 = node >> 2, draw = word node & 3): one Philox call serves four probes.
 enum : uint32_t { P_TARGET = 0, P_LOSS0 = 1, P_SCALAR = 2, P_TOPO = 3, P_PROXY = 4, P_LOSS = 5, P_RR = 6, P_CHURN = 7, P_TARGETS = 8, P_LOSSD = 9,
-                   P_PUSHPULL = 10 };
+                   P_PUSHPULL = 10, P_TOPOSYM = 11 };
 
 struct SimDev {
   uint32_t N, first, n, cap;

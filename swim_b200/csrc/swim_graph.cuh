@@ -160,8 +160,9 @@ int scan_u32(swim_sim *sim, Scratch &s, const uint32_t *in, size_t n, u64 *out) 
 
 // ------------------------------------------------------------------ stable radix sort by receiver
 // Digit counts of every tile, digit-major (hist[d * T + t]), so that one exclusive scan gives each (digit, tile) its first
-// output position. Keys equal to SWIM_NO_MEMBER (vacant slots of the id matrix) are left out.
-__global__ void __launch_bounds__(kGT) radix_hist_kernel(const uint32_t *key, size_t n, uint32_t shift, uint32_t *hist, uint32_t T) {
+// output position. With `skip`, keys equal to SWIM_NO_MEMBER (vacant slots of the id matrix) are left out.
+__global__ void __launch_bounds__(kGT) radix_hist_kernel(const uint32_t *key, size_t n, uint32_t shift, bool skip, uint32_t *hist,
+                                                         uint32_t T) {
   SWIM_SHARED_1D(uint32_t, s_h, kGT);
   for (uint32_t t = blockIdx.x; t < T; t += gridDim.x) {
     s_h[threadIdx.x] = 0;
@@ -170,7 +171,7 @@ __global__ void __launch_bounds__(kGT) radix_hist_kernel(const uint32_t *key, si
       const size_t i = (size_t)t * kTile + (size_t)k * kGT + threadIdx.x;
       if (i >= n) continue;
       const uint32_t x = key[i];
-      if (x != SWIM_NO_MEMBER) atomicAdd(&s_h[(x >> shift) & 255u], 1u);
+      if (!skip || x != SWIM_NO_MEMBER) atomicAdd(&s_h[(x >> shift) & 255u], 1u);
     }
     __syncthreads();
     hist[(size_t)threadIdx.x * T + t] = s_h[threadIdx.x];
@@ -182,7 +183,7 @@ __global__ void __launch_bounds__(kGT) radix_hist_kernel(const uint32_t *key, si
 // lanes with the same digit; CTA: thread d keeps the running count of digit d over the warps and rounds). vin == null:
 // the input is the id matrix itself and an element's value is its row (the sender).
 __global__ void __launch_bounds__(kGT) radix_scatter_kernel(const uint32_t *kin, const uint32_t *vin, uint32_t cap, size_t n,
-                                                            uint32_t shift, const u64 *off, uint32_t T, uint32_t *kout,
+                                                            uint32_t shift, bool skip, const u64 *off, uint32_t T, uint32_t *kout,
                                                             uint32_t *vout) {
   SWIM_SHARED_2D(uint32_t, s_cnt, kGW, kGT);
   SWIM_SHARED_2D(uint32_t, s_off, kGW, kGT);
@@ -197,7 +198,7 @@ __global__ void __launch_bounds__(kGT) radix_scatter_kernel(const uint32_t *kin,
     for (int k = 0; k < kItems; ++k) {
       const size_t i = (size_t)t * kTile + (size_t)k * kGT + threadIdx.x;
       const uint32_t key = i < n ? kin[i] : SWIM_NO_MEMBER;
-      const bool valid = key != SWIM_NO_MEMBER;
+      const bool valid = i < n && (!skip || key != SWIM_NO_MEMBER);
       const uint32_t dg = (key >> shift) & 255u;
       unsigned peers = __ballot_sync(kFull, valid);
       for (int b = 0; b < 8; ++b) {
@@ -224,25 +225,25 @@ __global__ void __launch_bounds__(kGT) radix_scatter_kernel(const uint32_t *kin,
   }
 }
 
-// Stable sort of the E keys of kin[0..cnt) that are not SWIM_NO_MEMBER (all < N), ascending; an element's value is its
-// position / cap. *key / *val point into scratch of `s`.
-int sort_by_key(swim_sim *sim, Scratch &s, const uint32_t *kin, size_t cnt, uint32_t cap, u64 E, uint32_t N, const uint32_t **key,
-                const uint32_t **val) {
+// Stable sort of the E keys of kin[0..cnt) (with `skip`: those that are not SWIM_NO_MEMBER) by their low `bits` bits,
+// ascending; an element's value is its position / cap. *key / *val point into scratch of `s`.
+int radix_sort(swim_sim *sim, Scratch &s, const uint32_t *kin, size_t cnt, uint32_t cap, u64 E, uint32_t bits, bool skip,
+               const uint32_t **key, const uint32_t **val) {
   uint32_t *kb[2], *vb[2], *hist;
   u64 *off;
   for (int b = 0; b < 2; ++b) { SCRATCH(s, kb[b], E); SCRATCH(s, vb[b], E); }
   const uint32_t T0 = (uint32_t)((cnt + kTile - 1) / kTile);
   SCRATCH(s, hist, (size_t)256 * T0);
   SCRATCH(s, off, (size_t)256 * T0 + 1);
-  const uint32_t bits = 32 - __builtin_clz(N - 1); // N >= 2 here: no key exists otherwise
   const uint32_t *vin = nullptr;
   int rc;
   for (uint32_t pass = 0; pass * 8 < bits; ++pass) {
     const uint32_t T = (uint32_t)((cnt + kTile - 1) / kTile), g = (uint32_t)grid_of(sim, T);
-    SWIM_LAUNCH(radix_hist_kernel, g, kGT, sim->stream, kin, cnt, pass * 8, hist, T);
+    SWIM_LAUNCH(radix_hist_kernel, g, kGT, sim->stream, kin, cnt, pass * 8, skip, hist, T);
     ++sim->launches;
     if ((rc = scan_u32(sim, s, hist, (size_t)256 * T, off))) return rc;
-    SWIM_LAUNCH(radix_scatter_kernel, g, kGT, sim->stream, kin, vin, cap, cnt, pass * 8, (const u64 *)off, T, kb[pass & 1], vb[pass & 1]);
+    SWIM_LAUNCH(radix_scatter_kernel, g, kGT, sim->stream, kin, vin, cap, cnt, pass * 8, skip, (const u64 *)off, T, kb[pass & 1],
+                vb[pass & 1]);
     ++sim->launches;
     GRAPH_TRY(sim, cudaGetLastError());
     kin = kb[pass & 1];
@@ -252,6 +253,13 @@ int sort_by_key(swim_sim *sim, Scratch &s, const uint32_t *kin, size_t cnt, uint
   *key = kin;
   *val = vin;
   return SWIM_OK;
+}
+
+// The E member ids of kin[0..cnt) (all < N; SWIM_NO_MEMBER entries left out), stably sorted.
+int sort_by_key(swim_sim *sim, Scratch &s, const uint32_t *kin, size_t cnt, uint32_t cap, u64 E, uint32_t N, const uint32_t **key,
+                const uint32_t **val) {
+  const uint32_t bits = 32 - __builtin_clz(N - 1); // N >= 2 here: no key exists otherwise
+  return radix_sort(sim, s, kin, cnt, cap, E, bits, true, key, val);
 }
 
 // ------------------------------------------------------------------ the graph

@@ -112,4 +112,6 @@ int coll_barrier(swim_sim *sim, unsigned long long mine = 0, unsigned long long 
 enum CollArray { kCollNbr, kCollVst, kCollVinc, kCollSelfInc };
 int coll_gather(swim_sim *sim, CollArray which, void *out);
 int coll_remap_eflag(swim_sim *sim, uint8_t *retired);
+// The argument checks every topology generator shares (swim_topology.cpp); *degree becomes N - 1 for the complete view.
+int topology_params(int kind, uint32_t N, uint32_t cap, uint32_t *degree);
 } // namespace swim

@@ -7,6 +7,19 @@
 
 #include "../../include/swim.h"
 
+namespace swim {
+// (declared in swim_host.h: swim_sim_generate_view checks its arguments here too)
+int topology_params(int kind, uint32_t N, uint32_t cap, uint32_t *degree) {
+  if (N == 0 || cap == 0 || cap % 32 || cap > SWIM_MAX_VIEW) return SWIM_EINVAL;
+  if (kind == SWIM_TOPO_COMPLETE) *degree = N - 1;
+  if (kind == SWIM_TOPO_SYMMETRIC && (N < 3 || *degree < 2 || *degree % 2)) return SWIM_EINVAL;
+  if (*degree > cap || *degree > N - 1) return SWIM_ECAP;
+  if (kind != SWIM_TOPO_COMPLETE && kind != SWIM_TOPO_RANDOM && kind != SWIM_TOPO_RING && kind != SWIM_TOPO_SYMMETRIC)
+    return SWIM_EINVAL;
+  return SWIM_OK;
+}
+} // namespace swim
+
 namespace {
 struct Philox {
   uint32_t k0, k1;
@@ -21,15 +34,50 @@ struct Philox {
     out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
   }
 };
+
+// Symmetric random views: the union of degree / 2 random Hamiltonian cycles. Cycle c visits the nodes in the order of
+// (key_c(i), i), key_c(i) = word i & 3 of Philox(ctr = (c, i >> 2, P_TOPOSYM = 11, 0)); each node takes its predecessor
+// and successor on every cycle, and its row is their distinct values, ascending. Written for clarity, not speed: this
+// is the statement the device generator (swim_topology.cuh) is tested against.
+void symmetric_rows(const Philox &rng, uint32_t N, uint32_t cap, uint32_t degree, uint32_t *out) {
+  const uint32_t cycles = degree / 2;
+#pragma omp parallel for schedule(dynamic, 1)
+  for (int64_t cc = 0; cc < (int64_t)cycles; ++cc) {
+    const uint32_t c = (uint32_t)cc;
+    std::vector<uint64_t> order(N);
+    for (uint32_t i = 0; i < N; ++i) {
+      uint32_t w[4];
+      rng(c, i >> 2, 11u, 0u, w);
+      order[i] = (uint64_t)w[i & 3] << 32 | i;
+    }
+    std::sort(order.begin(), order.end());
+    for (uint32_t t = 0; t < N; ++t) {
+      const uint32_t i = (uint32_t)order[t];
+      uint32_t *row = out + (size_t)i * cap;
+      row[2 * c] = (uint32_t)order[(t + N - 1) % N];
+      row[2 * c + 1] = (uint32_t)order[(t + 1) % N];
+    }
+  }
+#pragma omp parallel for schedule(static)
+  for (int64_t ii = 0; ii < (int64_t)N; ++ii) {
+    uint32_t *row = out + (size_t)ii * cap;
+    std::sort(row, row + degree);
+    const uint32_t cnt = (uint32_t)(std::unique(row, row + degree) - row);
+    for (uint32_t s = cnt; s < cap; ++s) row[s] = SWIM_NO_MEMBER;
+  }
+}
 } // namespace
 
 extern "C" int swim_topology_generate(int kind, uint32_t N, uint32_t cap, uint32_t degree, uint64_t seed,
                                       uint32_t *out) {
-  if (!out || N == 0 || cap == 0 || cap % 32 || cap > SWIM_MAX_VIEW) return SWIM_EINVAL;
-  if (kind == SWIM_TOPO_COMPLETE) degree = N - 1;
-  if (degree > cap || degree > N - 1) return SWIM_ECAP;
-  if (kind != SWIM_TOPO_COMPLETE && kind != SWIM_TOPO_RANDOM && kind != SWIM_TOPO_RING) return SWIM_EINVAL;
+  if (!out) return SWIM_EINVAL;
+  const int rc = swim::topology_params(kind, N, cap, &degree);
+  if (rc) return rc;
   const Philox rng{(uint32_t)seed, (uint32_t)(seed >> 32)};
+  if (kind == SWIM_TOPO_SYMMETRIC) {
+    symmetric_rows(rng, N, cap, degree, out);
+    return SWIM_OK;
+  }
 #pragma omp parallel for schedule(static)
   for (int64_t ii = 0; ii < (int64_t)N; ++ii) {
     const uint32_t i = (uint32_t)ii;

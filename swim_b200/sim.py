@@ -22,11 +22,15 @@ def default_config(**kw) -> A.Config:
     return cfg
 
 
+TOPOLOGIES = {"complete": A.TOPO_COMPLETE, "random": A.TOPO_RANDOM, "ring": A.TOPO_RING, "symmetric": A.TOPO_SYMMETRIC}
+
+
 def generate_topology(kind, n_nodes, view_cap=32, degree=32, seed=1):
-    """Synthetic view graph [N, view_cap] (ids ascending, NO_MEMBER padded). Host only."""
+    """Synthetic view graph [N, view_cap] (ids ascending, NO_MEMBER padded). Host only. kind: "complete", "random",
+    "ring", "symmetric" (the union of degree / 2 random Hamiltonian cycles: j lists i exactly when i lists j) or a
+    SWIM_TOPO_* number."""
     out = np.empty((n_nodes, view_cap), dtype=np.uint32)
-    kind = {"complete": A.TOPO_COMPLETE, "random": A.TOPO_RANDOM, "ring": A.TOPO_RING}.get(kind, kind)
-    check(lib().swim_topology_generate(kind, n_nodes, view_cap, degree, seed, out.ctypes.data),
+    check(lib().swim_topology_generate(TOPOLOGIES.get(kind, kind), n_nodes, view_cap, degree, seed, out.ctypes.data),
           "swim_topology_generate")
     return out
 
@@ -133,6 +137,13 @@ class Simulator:
         if nbr.size != self.cfg.n_nodes * self.cfg.view_cap:
             raise ValueError("nbr must be the global [N, view_cap] id matrix")
         check(lib().swim_sim_set_view(self._h, nbr.ctypes.data), "swim_sim_set_view", self._h)
+
+    def generate_view(self, kind, degree=32, seed=1):
+        """Generate the view graph on the device and install it as set_view does (swim_sim_generate_view): the matrix
+        generate_topology(kind, N, view_cap, degree, seed) returns, bit for bit, without a host copy. On a sharded handle
+        every rank generates the whole global matrix itself."""
+        check(lib().swim_sim_generate_view(self._h, TOPOLOGIES.get(kind, kind), degree, seed), "swim_sim_generate_view",
+              self._h)
 
     def remove_dead_nodes(self, min_age=0):
         """removeDeadNodes (Core.hs:65-67) on every local store: Dead entries at least `min_age` rounds old leave.
