@@ -10,7 +10,7 @@
 -- Drop this module into src/, add `extra-libraries: swim_b200` to swim.cabal, and Core.hs's functions
 -- can delegate to the accelerated implementation (section 3 of INTEGRATION.md).
 module SwimFFI
-  ( Sim, CConfig(..), CMember(..), CMessage(..), CGossip(..)
+  ( Sim, CConfig(..), CMember(..), CMessage(..), CGossip(..), CJoin(..)
   , defaultConfig, simCreate, simDestroy, simSetView, simStep, simDigest, simMismatches
   , getMembers, setMembers, kRandomMembers, removeDeadNodes, nextSeqNo, nextIncarnation
   , suspectNode, deadNode, aliveNode, handleMessage, broadcast
@@ -20,6 +20,8 @@ module SwimFFI
   , c_simInjectDatagram, c_getBroadcasts, c_takeBroadcasts, c_tickTimers, c_envEncode, c_envDecode, simCounters
     -- bulk membership edits between steps: removeDeadNodes / addNewMember on every store at once
   , c_simRemoveDeadNodes, c_simAddMembers
+    -- seed joins between steps: Join(joinHosts) for many processes at once
+  , simJoin, joinFresh, c_simJoin
   ) where
 
 import Control.Monad (when)
@@ -105,6 +107,15 @@ instance Storable CGossip where
     fillBytes p 0 56
     pokeByteOff p 0 gIsDirect; pokeByteOff p 2 gDestPort; pokeByteOff p 4 gDestAddr; poke (p `plusPtr` 8) gMsg
 
+-- | swim_join_t: one joiner and one of its join hosts (Config.joinHosts, Types.hs:47)
+data CJoin = CJoin { jNode, jSeed :: !Word32 } deriving (Eq, Show)
+
+instance Storable CJoin where
+  sizeOf _ = 8
+  alignment _ = 4
+  peek p = CJoin <$> peekByteOff p 0 <*> peekByteOff p 4
+  poke p CJoin{..} = pokeByteOff p 0 jNode >> pokeByteOff p 4 jSeed
+
 foreign import ccall unsafe "swim_config_default"    c_configDefault :: Ptr CConfig -> IO CInt
 foreign import ccall safe   "swim_sim_create"        c_simCreate     :: Ptr CConfig -> Ptr Sim -> IO CInt
 foreign import ccall safe   "swim_sim_destroy"       simDestroy      :: Sim -> IO ()
@@ -146,6 +157,8 @@ foreign import ccall safe   "swim_sim_remove_dead_nodes" c_simRemoveDeadNodes ::
 foreign import ccall safe   "swim_sim_add_members"     c_simAddMembers     :: Sim -> Ptr Word32 -> CSize -> Ptr Word64 -> Ptr Word64 -> IO CInt
 -- push-pull anti-entropy between steps (memberlist; joinHosts, Types.hs:47, completed): exchanges, inserted, full
 foreign import ccall safe   "swim_sim_push_pull"       c_simPushPull       :: Sim -> Ptr Word64 -> Ptr Word64 -> Ptr Word64 -> IO CInt
+-- seed joins between steps (Config.joinHosts, Types.hs:47; Util.hs:46): pairs, count, flags; exchanges, inserted, full
+foreign import ccall safe   "swim_sim_join"            c_simJoin           :: Sim -> Ptr CJoin -> CSize -> Word32 -> Ptr Word64 -> Ptr Word64 -> Ptr Word64 -> IO CInt
 -- the view graph generated on the device (kind = SWIM_TOPO_*, degree, seed) and installed as by swim_sim_set_view_device
 foreign import ccall safe   "swim_sim_generate_view"   c_simGenerateView   :: Sim -> CInt -> Word32 -> Word64 -> IO CInt
 foreign import ccall unsafe "swim_envelope_encode"     c_envEncode         :: Ptr () -> CSize -> Ptr Word8 -> CSize -> Ptr CSize -> IO CInt
@@ -220,3 +233,14 @@ handleMessage sim node (addr, port) msg = with msg $ \pm -> allocaArray 2 $ \out
 
 broadcast :: Sim -> Word32 -> CMessage -> IO ()                     -- disseminate, Broadcast branch (Core.hs:131,136-138)
 broadcast sim node msg = with msg $ \pm -> c_broadcast sim node pm >>= orFail sim
+
+-- | SWIM_JOIN_FRESH: the joiners restart empty before they join.
+joinFresh :: Word32
+joinFresh = 1
+
+-- | Join(joinHosts) for many processes at once, between steps: each (node, host) pair is one full-state exchange.
+-- Returns (exchanges, inserted, full).
+simJoin :: Sim -> Word32 -> [CJoin] -> IO (Word64, Word64, Word64)
+simJoin sim flags js = withArrayLen js $ \n pj -> alloca $ \pe -> alloca $ \pn -> alloca $ \pf -> do
+  c_simJoin sim pj (fromIntegral n) flags pe pn pf >>= orFail sim
+  (,,) <$> peek pe <*> peek pn <*> peek pf

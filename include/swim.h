@@ -353,6 +353,28 @@ int swim_sim_add_members(swim_sim_t *sim, const swim_member_add_t *adds, size_t 
  * dropped on a full row. */
 int swim_sim_push_pull(swim_sim_t *sim, uint64_t *n_exchanges, uint64_t *n_inserted, uint64_t *n_full);
 
+/* Seed joins between steps (DESIGN.md §2.7): memberlist's Join(joinHosts), the join the reference names and never
+ * performs (Config.joinHosts, Types.hs:47, default udp://127.0.0.1:4000 at Util.hs:46). At the current round (the round
+ * counter does not advance) each pair {node j, seed s} is one full-state exchange between j and its join host s, with
+ * the push-pull exchange's records and merge rules. A pair is an exchange iff both are up; neither needs to list the
+ * other, and either may have an empty row. A receiver merges its distinct senders (the seeds of its exchanges and the
+ * joiners that named it) once each, in ascending id. With SWIM_JOIN_FRESH every listed joiner that is up first loses its
+ * whole view and piggyback buffer (self_inc is kept): a process that restarts empty, so it sends only Alive(self). Every
+ * pair is checked before anything changes (ids < N, node != seed; SWIM_EINVAL otherwise); n = 0 is a no-op. No random
+ * draws: the result is a function of the pairs, the state and the round. SWIM_ESTATE as for swim_sim_push_pull. On a
+ * sharded handle a collective: every rank is given the same global list; outputs are this rank's (the pairs whose joiner
+ * it owns, its receivers' inserts and drops), their sums the single-shard ones. The view is marked changed as by the
+ * bulk edits when some rank inserted a member or a fresh reset emptied an occupied slot; otherwise only state changes
+ * and the checkpoint stays valid.
+ * Outputs may be NULL: *n_exchanges = pairs that were exchanges (duplicates included), *n_inserted = members inserted,
+ * *n_full = inserts dropped on a full row. */
+typedef struct swim_join {
+  uint32_t node, seed;
+} swim_join_t;
+enum { SWIM_JOIN_FRESH = 1u << 0 };
+int swim_sim_join(swim_sim_t *sim, const swim_join_t *joins, size_t n, uint32_t flags, uint64_t *n_exchanges,
+                  uint64_t *n_inserted, uint64_t *n_full);
+
 /* Bulk copies of one state array (SWIM_ARR_*) between device and a host buffer of exactly
  * `bytes` bytes. set_array(SWIM_ARR_NBR) is rejected: use swim_sim_set_view. */
 int swim_sim_get_array(swim_sim_t *sim, int arr, void *host_buf, size_t bytes);

@@ -41,6 +41,11 @@ def main():
     ap.add_argument("--push-pull-every", type=int, default=0, metavar="R",
                     help="a push-pull state exchange (memberlist anti-entropy) after every R-th round (a collective "
                          "on several GPUs)")
+    ap.add_argument("--join-hosts", type=int, default=0, metavar="K",
+                    help="K join hosts drawn once from the seed: after every step chunk each process that restarted in "
+                         "it joins through all K (memberlist's Join(joinHosts); a collective on several GPUs)")
+    ap.add_argument("--join-fresh", action="store_true",
+                    help="the restarted processes lose their view and piggyback buffer before joining")
     ap.add_argument("--seed", type=int, default=0x5EED0001 + 5)
     args = ap.parse_args()
 
@@ -65,22 +70,33 @@ def main():
 
     cfg = default_config(n_nodes=n, suspicion_rounds=args.suspicion[0], loss_ppm=args.loss_ppm, seed=args.seed, rank=rank,
                          world=world, device=local, flags=args.flags, churn_ppm=args.crash_ppm, rejoin_min=10, rejoin_max=50)
-    t0 = time.perf_counter()
-    sim = Simulator(cfg)
-    t1 = time.perf_counter()
-    sim.generate_view(args.topology, 32, seed=args.seed & 0xFFFF)  # every rank generates the global matrix on its GPU
-    t_topo = time.perf_counter() - t1
-    mode = sd.connect(sim)
-    sim.save()
-    t_setup = time.perf_counter() - t0 - t_topo
-    for S in args.suspicion:
+    def setup():
+        t0 = time.perf_counter()
+        sim = Simulator(cfg)
+        t1 = time.perf_counter()
+        sim.generate_view(args.topology, 32, seed=args.seed & 0xFFFF)  # every rank generates the global matrix on its GPU
+        t_topo = time.perf_counter() - t1
+        mode = sd.connect(sim)
+        sim.save()
+        return sim, mode, t_topo, time.perf_counter() - t0 - t_topo
+
+    sim, mode, t_topo, t_setup = setup()
+    hosts = None
+    if args.join_hosts:  # the same draw on every rank
+        import numpy as np
+        hosts = np.sort(np.random.default_rng(args.seed).choice(n, size=args.join_hosts, replace=False)).astype(np.uint32)
+    for k, S in enumerate(args.suspicion):
         barrier()
+        if k and args.join_hosts:  # a join that changed memberships dropped the checkpoint
+            sim.close()
+            sim, mode, t_topo, t_setup = setup()
         sim.load()
         smax = max(args.suspicion_max, S) if args.suspicion_max else 0
         sim.set_params(suspicion_rounds=S, suspicion_max=min(smax, 15))
         barrier()
         t0 = time.perf_counter()
-        res = run_sweep_point(sim, None, args.rounds, args.sample_every, red, args.push_pull_every)
+        res = run_sweep_point(sim, None, args.rounds, args.sample_every, red, args.push_pull_every, hosts,
+                              args.join_fresh)
         wall = time.perf_counter() - t0
         if rank == 0:
             rep = res["report"]
@@ -99,6 +115,9 @@ def main():
             if args.push_pull_every:
                 line["config"]["push_pull_every"] = args.push_pull_every
                 line["push_pull"] = res["push_pull"]
+            if args.join_hosts:
+                line["config"].update(join_hosts=hosts.tolist(), join_fresh=args.join_fresh)
+                line["join"] = res["join"]
             print(json.dumps(line), flush=True)
     sim.close()
     if world > 1:

@@ -21,6 +21,7 @@ IPC_BLOB_BYTES = 1024
 EV_CRASH, EV_REJOIN, EV_INJECT = 0, 1, 2
 F_NONE, F_STRICT_OVERRIDE, F_ROUND_ROBIN = 0, 1, 2  # SWIM_F_*: protocol variants
 TOPO_COMPLETE, TOPO_RANDOM, TOPO_RING, TOPO_SYMMETRIC = 0, 1, 2, 3
+JOIN_FRESH = 1  # SWIM_JOIN_FRESH: swim_sim_join empties the joiners first
 
 (ARR_ALIVE, ARR_SELF_INC, ARR_SEQNO, ARR_NBR, ARR_VST, ARR_VINC, ARR_VLAST, ARR_PB, ARR_PB_CNT, ARR_BACK_AT,
  ARR_LAST_CRASH, ARR_LAST_REJOIN) = range(12)
@@ -73,6 +74,10 @@ class MemberAdd(C.Structure):
     _fields_ = [("observer", C.c_uint32), ("member", C.c_uint32), ("incarnation", C.c_uint32), ("_pad", C.c_uint32)]
 
 
+class Join(C.Structure):
+    _fields_ = [("node", C.c_uint32), ("seed", C.c_uint32)]
+
+
 class Datagram(C.Structure):
     _fields_ = [("src", C.c_uint32), ("dst", C.c_uint32), ("length", C.c_uint32), ("n_messages", C.c_uint32),
                 ("offset", C.c_uint64)]
@@ -95,6 +100,7 @@ EVENT_DTYPE = _np.dtype({"names": ["round", "node", "kind", "msg_kind", "msg_nod
                          "offsets": [0, 4, 8, 16, 24, 32, 40],
                          "itemsize": C.sizeof(Event)})
 MEMBER_ADD_DTYPE = _np.dtype([("observer", "<u4"), ("member", "<u4"), ("incarnation", "<u4"), ("_pad", "<u4")])
+JOIN_DTYPE = _np.dtype([("node", "<u4"), ("seed", "<u4")])
 ARRAY_DTYPES = {
     ARR_ALIVE: _np.dtype("u1"), ARR_SELF_INC: _np.dtype("<u4"), ARR_SEQNO: _np.dtype("<u4"),
     ARR_NBR: _np.dtype("<u4"), ARR_VST: _np.dtype("u1"), ARR_VINC: _np.dtype("<u4"),

@@ -84,12 +84,14 @@ __global__ void __launch_bounds__(kThreads) push_pull_kernel(SimDev d, uint32_t 
     uint32_t self_inc = d.self_inc[j];
     const uint32_t self_inc0 = self_inc;
     bool grew = false;
-    for (;;) {
+    for (uint32_t prev = SWIM_NO_MEMBER;;) {
       const uint32_t ch = x < x1 ? chooser[x] : SWIM_NO_MEMBER;
       uint32_t s;
       if (pull != SWIM_NO_MEMBER && pull <= ch) { s = pull; pull = SWIM_NO_MEMBER; if (ch == s) ++x; }
       else if (ch != SWIM_NO_MEMBER) { s = ch; ++x; }
       else break;
+      if (s == prev) continue; // a join's chooser list may repeat a sender (duplicated pairs): it is merged once
+      prev = s;
       // the sender's row, lane-owned like the receiver's
       uint32_t snb[W], sst[W], sinc[W];
       int nocc = 0; // occupied slots (vacancies are last)
@@ -158,11 +160,44 @@ __global__ void __launch_bounds__(kThreads) push_pull_kernel(SimDev d, uint32_t 
 } // namespace
 
 namespace {
+// The snapshot of a single shard: copies of its rows and incarnations, taken on the stream before any row changes.
+int pp_snapshot(swim_sim *sim, Scratch &s, PpSnap *snap) {
+  const SimDev &d = sim->dev;
+  const size_t n = d.n, slots = n * d.cap;
+  uint32_t *nb, *vi, *si;
+  uint8_t *vs;
+  SCRATCH(s, nb, slots);
+  SCRATCH(s, vi, slots);
+  SCRATCH(s, si, n);
+  SCRATCH(s, vs, slots);
+  GRAPH_TRY(sim, cudaMemcpyAsync(nb, d.nbr, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
+  GRAPH_TRY(sim, cudaMemcpyAsync(vi, d.vinc, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
+  GRAPH_TRY(sim, cudaMemcpyAsync(si, d.self_inc, n * 4, cudaMemcpyDeviceToDevice, sim->stream));
+  GRAPH_TRY(sim, cudaMemcpyAsync(vs, d.vst, slots, cudaMemcpyDeviceToDevice, sim->stream));
+  snap->nbr = nb; snap->vinc = vi; snap->self_inc = si; snap->vst = vs;
+  return SWIM_OK;
+}
+
+// push_pull_kernel at the handle's row width: every local receiver j merges {part[j]} and chooser[seg[j] .. seg[j + 1]).
+int pp_merge(swim_sim *sim, const PpSnap &snap, const uint32_t *part, const u64 *seg, const uint32_t *chooser, u64 *res) {
+  const SimDev &d = sim->dev;
+  const int g = grid_of(sim, (d.n + kWarpsPerBlock - 1) / kWarpsPerBlock);
+  switch (d.cap / 32) {
+    case 1: SWIM_LAUNCH(push_pull_kernel<1>, g, kThreads, sim->stream, d, sim->round, snap, part, seg, chooser, res); break;
+    case 2: SWIM_LAUNCH(push_pull_kernel<2>, g, kThreads, sim->stream, d, sim->round, snap, part, seg, chooser, res); break;
+    case 4: SWIM_LAUNCH(push_pull_kernel<4>, g, kThreads, sim->stream, d, sim->round, snap, part, seg, chooser, res); break;
+    default: SWIM_LAUNCH(push_pull_kernel<8>, g, kThreads, sim->stream, d, sim->round, snap, part, seg, chooser, res); break;
+  }
+  ++sim->launches;
+  GRAPH_TRY(sim, cudaGetLastError());
+  return SWIM_OK;
+}
+
 // The exchange on this shard's receivers. Sharded: between the gather barriers of swim_sim_push_pull, with `snap` the
 // gathered global snapshot. h = {inserted, dropped on a full row, exchanges} of this shard.
 int push_pull_local(swim_sim *sim, Scratch &s, const PpSnap *gsnap, u64 h[3]) {
   const SimDev &d = sim->dev;
-  const size_t n = d.n, slots = n * d.cap;
+  const size_t n = d.n;
   const uint32_t rows = gsnap ? d.N : d.n; // the rows the partners are drawn from
   uint32_t *part, *cnt, *key = nullptr;
   u64 *seg, *res, E = 0, ex = 0;
@@ -189,35 +224,35 @@ int push_pull_local(swim_sim *sim, Scratch &s, const PpSnap *gsnap, u64 h[3]) {
     const uint32_t *skey, *chooser = nullptr;
     if (E && (rc = sort_by_key(sim, s, key ? key : part, rows, 1, E, d.N, &skey, &chooser))) return rc;
     PpSnap snap;
-    if (gsnap) {
-      snap = *gsnap;
-    } else {
-      uint32_t *nb, *vi, *si;
-      uint8_t *vs;
-      SCRATCH(s, nb, slots);
-      SCRATCH(s, vi, slots);
-      SCRATCH(s, si, n);
-      SCRATCH(s, vs, slots);
-      GRAPH_TRY(sim, cudaMemcpyAsync(nb, d.nbr, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
-      GRAPH_TRY(sim, cudaMemcpyAsync(vi, d.vinc, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
-      GRAPH_TRY(sim, cudaMemcpyAsync(si, d.self_inc, n * 4, cudaMemcpyDeviceToDevice, sim->stream));
-      GRAPH_TRY(sim, cudaMemcpyAsync(vs, d.vst, slots, cudaMemcpyDeviceToDevice, sim->stream));
-      snap.nbr = nb; snap.vinc = vi; snap.self_inc = si; snap.vst = vs;
-    }
-    const int g = grid_of(sim, (n + kWarpsPerBlock - 1) / kWarpsPerBlock);
-    const uint32_t *cp = part;
-    const u64 *cs = seg;
-    switch (d.cap / 32) {
-      case 1: SWIM_LAUNCH(push_pull_kernel<1>, g, kThreads, sim->stream, d, sim->round, snap, cp, cs, chooser, res); break;
-      case 2: SWIM_LAUNCH(push_pull_kernel<2>, g, kThreads, sim->stream, d, sim->round, snap, cp, cs, chooser, res); break;
-      case 4: SWIM_LAUNCH(push_pull_kernel<4>, g, kThreads, sim->stream, d, sim->round, snap, cp, cs, chooser, res); break;
-      default: SWIM_LAUNCH(push_pull_kernel<8>, g, kThreads, sim->stream, d, sim->round, snap, cp, cs, chooser, res); break;
-    }
-    ++sim->launches;
-    GRAPH_TRY(sim, cudaGetLastError());
+    if (gsnap) snap = *gsnap;
+    else if ((rc = pp_snapshot(sim, s, &snap))) return rc;
+    if ((rc = pp_merge(sim, snap, part, seg, chooser, res))) return rc;
   }
   GRAPH_TRY(sim, cudaMemcpyAsync(h, res, 3 * sizeof(u64), cudaMemcpyDeviceToHost, sim->stream));
   GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
+  return SWIM_OK;
+}
+
+// Sharded: device buffers for the global snapshot, [world * per] rows addressed by global id ...
+int pp_gather_alloc(swim_sim *sim, Scratch &s, PpSnap *snap) {
+  const SimDev &d = sim->dev;
+  const size_t rows = (size_t)d.world * d.per, gslots = rows * d.cap;
+  uint32_t *nb, *vi, *si;
+  uint8_t *vs;
+  SCRATCH(s, nb, gslots);
+  SCRATCH(s, vi, gslots);
+  SCRATCH(s, si, rows);
+  SCRATCH(s, vs, gslots);
+  snap->nbr = nb; snap->vinc = vi; snap->self_inc = si; snap->vst = vs;
+  return SWIM_OK;
+}
+
+// ... and every rank's rows and incarnations gathered into them (between barriers: no rank changes a row meanwhile).
+int pp_gather(swim_sim *sim, const PpSnap &snap) {
+  int rc;
+  if ((rc = coll_gather(sim, kCollNbr, (void *)snap.nbr)) || (rc = coll_gather(sim, kCollVst, (void *)snap.vst)) ||
+      (rc = coll_gather(sim, kCollVinc, (void *)snap.vinc)) || (rc = coll_gather(sim, kCollSelfInc, (void *)snap.self_inc)))
+    return rc;
   return SWIM_OK;
 }
 
@@ -227,24 +262,14 @@ int push_pull_local(swim_sim *sim, Scratch &s, const PpSnap *gsnap, u64 h[3]) {
 // that barrier: a peer that shares this device may start its round kernels right after it, and cudaFree would wait for
 // them while they wait for this rank.
 int push_pull_sharded(swim_sim *sim, u64 h[3], u64 *inserted_all) {
-  const SimDev &d = sim->dev;
-  const size_t rows = (size_t)d.world * d.per, gslots = rows * d.cap;
   int rc;
   {
     Scratch s(sim);
-    uint32_t *nb, *vi, *si;
-    uint8_t *vs;
-    SCRATCH(s, nb, gslots);
-    SCRATCH(s, vi, gslots);
-    SCRATCH(s, si, rows);
-    SCRATCH(s, vs, gslots);
-    if ((rc = coll_barrier(sim))) return rc;
-    if ((rc = coll_gather(sim, kCollNbr, nb)) || (rc = coll_gather(sim, kCollVst, vs)) ||
-        (rc = coll_gather(sim, kCollVinc, vi)) || (rc = coll_gather(sim, kCollSelfInc, si)))
-      return rc;
-    if ((rc = coll_barrier(sim))) return rc;
     PpSnap snap;
-    snap.nbr = nb; snap.vinc = vi; snap.self_inc = si; snap.vst = vs;
+    if ((rc = pp_gather_alloc(sim, s, &snap))) return rc;
+    if ((rc = coll_barrier(sim))) return rc;
+    if ((rc = pp_gather(sim, snap))) return rc;
+    if ((rc = coll_barrier(sim))) return rc;
     if ((rc = push_pull_local(sim, s, &snap, h))) return rc;
   }
   return coll_barrier(sim, h[0], inserted_all);

@@ -304,6 +304,8 @@ extern "C" int swim_sim_local_range(const swim_sim_t *sim, uint32_t *first, uint
 #include "swim_graph.cuh"
 // swim_sim_push_pull: the state exchange between steps
 #include "swim_pushpull.cuh"
+// swim_sim_join: seed joins between steps
+#include "swim_join.cuh"
 // swim_sim_generate_view: the synthetic view graphs generated on the device
 #include "swim_topology.cuh"
 

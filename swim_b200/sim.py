@@ -176,6 +176,21 @@ class Simulator:
         check(lib().swim_sim_push_pull(self._h, C.byref(e), C.byref(n), C.byref(f)), "swim_sim_push_pull", self._h)
         return e.value, n.value, f.value
 
+    def join(self, nodes, seeds, fresh=False):
+        """Seed joins (DESIGN.md 2.7) at the current round, memberlist's Join(joinHosts): pair k is one full-state
+        exchange between joiner nodes[k] and its join host seeds[k] when both are up, whether or not either lists the
+        other; each side merges what it receives as push_pull does. With `fresh` every listed joiner that is up first
+        loses its view and piggyback buffer (a restart that lost its state). Returns (exchanges, inserted, full) of this
+        shard. On a sharded handle a collective: every rank is given the same global list."""
+        nodes = np.atleast_1d(np.asarray(nodes))
+        pairs = np.zeros(len(nodes), dtype=A.JOIN_DTYPE)
+        pairs["node"] = nodes
+        pairs["seed"] = seeds
+        e, n, f = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        check(lib().swim_sim_join(self._h, pairs.ctypes.data, len(pairs), A.JOIN_FRESH if fresh else 0, C.byref(e),
+                                  C.byref(n), C.byref(f)), "swim_sim_join", self._h)
+        return e.value, n.value, f.value
+
     def inject(self, events):
         events = np.ascontiguousarray(events, dtype=A.EVENT_DTYPE)
         check(lib().swim_sim_inject(self._h, events.ctypes.data, len(events)), "swim_sim_inject", self._h)

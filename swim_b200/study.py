@@ -11,6 +11,8 @@ Terms, per view entry (observer i, member m) of a live observer:
                `stale_dead_up` = Dead since before the member's last rejoin (the Alive(inc+1) has not arrived).
 The mismatch count of the library (`swim_sim_mismatches`) counts every entry that disagrees with the truth, i.e.
 undetected + suspected + false_dead + stale_dead_up (a Dead entry of a down member agrees, stale or not)."""
+import time
+
 import numpy as np
 
 from . import _abi as A
@@ -94,16 +96,35 @@ def latency_stats(hist):
             "max": int(np.flatnonzero(hist)[-1])}
 
 
-def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None, push_pull_every=0):
+def restart_joins(sim, hosts, since, upto):
+    """memberlist's restart, Join(joinHosts): every up process whose last rejoin lies in rounds (since, upto] paired with
+    each join host (never with itself). Built from the replicated SWIM_ARR_ALIVE / SWIM_ARR_LAST_REJOIN arrays, so every
+    rank builds the same list. Returns (nodes, seeds)."""
+    hosts = np.asarray(hosts, dtype=np.uint32)
+    alive = sim.get_array(A.ARR_ALIVE).astype(bool)
+    back = sim.get_array(A.ARR_LAST_REJOIN).astype(np.int64)
+    who = np.flatnonzero(alive & (back > since) & (back <= upto)).astype(np.uint32)
+    nodes, seeds = np.repeat(who, len(hosts)), np.tile(hosts, len(who))
+    keep = nodes != seeds
+    return nodes[keep], seeds[keep]
+
+
+def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None, push_pull_every=0, join_hosts=None,
+                    join_fresh=False):
     """Step `rounds` rounds, sampling the convergence count; returns the time series, the final counters and the final
     view report. `reduce_sum(list_of_numbers) -> list` adds values over ranks (identity for one GPU). push_pull_every = R
     > 0: a push-pull state exchange (Simulator.push_pull; on a sharded handle a collective, which every rank reaches at
-    the same round) after every R-th round; its outputs, summed over the calls and the ranks, are in "push_pull"."""
+    the same round) after every R-th round; its outputs, summed over the calls and the ranks, are in "push_pull".
+    join_hosts = the ids of K join hosts: after every step chunk the processes that restarted in it join through all K
+    (Simulator.join, `fresh` = join_fresh: the restart lost its state; a collective on a sharded handle). The summed
+    outputs, the joins and the host time of the calls are in "join"."""
     red = reduce_sum or (lambda xs: xs)
     series = []
     done = 0
     device_ms = 0.0
     pp = [0, 0, 0]
+    jn = [0, 0, 0, 0]  # exchanges, inserted, full, pairs
+    join_s = 0.0
     while done < rounds:
         step = min(sample_every - done % sample_every, rounds - done)
         if push_pull_every:
@@ -112,6 +133,12 @@ def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None, push_
         if hasattr(sim, "last_step_ms"):
             device_ms += float(sim.last_step_ms())  # CUDA events around the call's kernels, this rank
         done += step
+        if join_hosts is not None and len(join_hosts):
+            nodes, seeds = restart_joins(sim, join_hosts, done - step, done)
+            t0 = time.perf_counter()
+            got = sim.join(nodes, seeds, join_fresh)  # (returns after a device synchronisation)
+            join_s += time.perf_counter() - t0
+            jn = [a + b for a, b in zip(jn, list(got) + [len(nodes)])]
         if push_pull_every and done % push_pull_every == 0:
             pp = [a + b for a, b in zip(pp, sim.push_pull())]
         if done % sample_every == 0 or done == rounds:
@@ -127,4 +154,7 @@ def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None, push_
            "device_ms": device_ms, "device_us_per_round": device_ms * 1e3 / max(1, rounds)}
     if push_pull_every:
         out["push_pull"] = dict(zip(("exchanges", "inserted", "full"), (int(v) for v in red(pp))))
+    if join_hosts is not None and len(join_hosts):
+        out["join"] = dict(zip(("exchanges", "inserted", "full"), (int(v) for v in red(jn[:3]))))
+        out["join"].update(pairs=jn[3], host_s_rank0=join_s)
     return out
