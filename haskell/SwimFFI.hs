@@ -22,6 +22,8 @@ module SwimFFI
   , c_simRemoveDeadNodes, c_simAddMembers
     -- seed joins between steps: Join(joinHosts) for many processes at once
   , simJoin, joinFresh, c_simJoin
+    -- graceful leaves between steps: memberlist's Leave for many processes at once
+  , simLeave, c_simLeave
   ) where
 
 import Control.Monad (when)
@@ -159,6 +161,8 @@ foreign import ccall safe   "swim_sim_add_members"     c_simAddMembers     :: Si
 foreign import ccall safe   "swim_sim_push_pull"       c_simPushPull       :: Sim -> Ptr Word64 -> Ptr Word64 -> Ptr Word64 -> IO CInt
 -- seed joins between steps (Config.joinHosts, Types.hs:47; Util.hs:46): pairs, count, flags; exchanges, inserted, full
 foreign import ccall safe   "swim_sim_join"            c_simJoin           :: Sim -> Ptr CJoin -> CSize -> Word32 -> Ptr Word64 -> Ptr Word64 -> Ptr Word64 -> IO CInt
+-- graceful leaves between steps (memberlist's Leave; the reference has none): ids, count; left, delivered
+foreign import ccall safe   "swim_sim_leave"           c_simLeave          :: Sim -> Ptr Word32 -> CSize -> Ptr Word64 -> Ptr Word64 -> IO CInt
 -- the view graph generated on the device (kind = SWIM_TOPO_*, degree, seed) and installed as by swim_sim_set_view_device
 foreign import ccall safe   "swim_sim_generate_view"   c_simGenerateView   :: Sim -> CInt -> Word32 -> Word64 -> IO CInt
 foreign import ccall unsafe "swim_envelope_encode"     c_envEncode         :: Ptr () -> CSize -> Ptr Word8 -> CSize -> Ptr CSize -> IO CInt
@@ -244,3 +248,10 @@ simJoin :: Sim -> Word32 -> [CJoin] -> IO (Word64, Word64, Word64)
 simJoin sim flags js = withArrayLen js $ \n pj -> alloca $ \pe -> alloca $ \pn -> alloca $ \pf -> do
   c_simJoin sim pj (fromIntegral n) flags pe pn pf >>= orFail sim
   (,,) <$> peek pe <*> peek pn <*> peek pf
+
+-- | memberlist's Leave for many processes at once, between steps: each listed process that is up goes down and its
+-- members receive Dead about it, from it. Returns (left, delivered).
+simLeave :: Sim -> [Word32] -> IO (Word64, Word64)
+simLeave sim ids = withArrayLen ids $ \n pi' -> alloca $ \pl -> alloca $ \pd -> do
+  c_simLeave sim pi' (fromIntegral n) pl pd >>= orFail sim
+  (,) <$> peek pl <*> peek pd

@@ -375,6 +375,21 @@ enum { SWIM_JOIN_FRESH = 1u << 0 };
 int swim_sim_join(swim_sim_t *sim, const swim_join_t *joins, size_t n, uint32_t flags, uint64_t *n_exchanges,
                   uint64_t *n_inserted, uint64_t *n_full);
 
+/* Graceful leaves between steps (DESIGN.md §2.8): memberlist's Leave, a dead message about the departing process whose
+ * From is the process itself, broadcast before it stops. The reference has no leave: every departure is a failure that
+ * the others must detect. At the current round (the round counter does not advance; no random draws) the leavers are the
+ * distinct listed ids that are up (a repeated id leaves once, a down id is ignored). Every leaver goes down as by a
+ * SWIM_EV_CRASH at this round (alive = 0, last_crash = round) and back_at = 0, so the seeded churn never brings it back
+ * (a SWIM_EV_REJOIN does, with self_inc + 1). Its row, buffer and self_inc are kept. Then each member m that leaver L
+ * holds Alive or Suspect and that is up receives Dead(self_inc_L, L, from = L), handled exactly as a SWIM_EV_INJECT
+ * datagram at this round; a recipient applies its leavers' records in ascending leaver id. The gossip memberlist's Leave
+ * waits for is condensed into the call: a "flushed" leave. No membership changes: the mail graph and the checkpoint stay
+ * valid. Every id is checked before anything changes (id < N, at most 2^31 - 1 ids; SWIM_EINVAL otherwise); n = 0 is a
+ * no-op. SWIM_ESTATE as for swim_sim_join. On a sharded handle a collective: every rank is given the same global list;
+ * outputs are this rank's (the leavers it owns, its recipients' records), their sums the single-shard ones.
+ * Outputs may be NULL: *n_left = leavers, *n_delivered = (recipient, leaver) records applied or rejected. */
+int swim_sim_leave(swim_sim_t *sim, const uint32_t *nodes, size_t n, uint64_t *n_left, uint64_t *n_delivered);
+
 /* Bulk copies of one state array (SWIM_ARR_*) between device and a host buffer of exactly
  * `bytes` bytes. set_array(SWIM_ARR_NBR) is rejected: use swim_sim_set_view. */
 int swim_sim_get_array(swim_sim_t *sim, int arr, void *host_buf, size_t bytes);

@@ -46,6 +46,9 @@ def main():
                          "it joins through all K (memberlist's Join(joinHosts); a collective on several GPUs)")
     ap.add_argument("--join-fresh", action="store_true",
                     help="the restarted processes lose their view and piggyback buffer before joining")
+    ap.add_argument("--leave-ppm", type=int, default=0, metavar="P",
+                    help="after every step chunk each up process leaves gracefully (memberlist's Leave) with "
+                         "probability P / 10^6, the same draw on every rank and for every S (a collective on several GPUs)")
     ap.add_argument("--seed", type=int, default=0x5EED0001 + 5)
     args = ap.parse_args()
 
@@ -96,7 +99,7 @@ def main():
         barrier()
         t0 = time.perf_counter()
         res = run_sweep_point(sim, None, args.rounds, args.sample_every, red, args.push_pull_every, hosts,
-                              args.join_fresh)
+                              args.join_fresh, args.leave_ppm)
         wall = time.perf_counter() - t0
         if rank == 0:
             rep = res["report"]
@@ -118,6 +121,9 @@ def main():
             if args.join_hosts:
                 line["config"].update(join_hosts=hosts.tolist(), join_fresh=args.join_fresh)
                 line["join"] = res["join"]
+            if args.leave_ppm:
+                line["config"]["leave_ppm"] = args.leave_ppm
+                line["leave"] = res["leave"]
             print(json.dumps(line), flush=True)
     sim.close()
     if world > 1:

@@ -49,6 +49,7 @@ def lib():
     sig("swim_sim_add_members", i, vp, vp, sz, P(u64), P(u64))
     sig("swim_sim_push_pull", i, vp, P(u64), P(u64), P(u64))
     sig("swim_sim_join", i, vp, vp, sz, u32, P(u64), P(u64), P(u64))
+    sig("swim_sim_leave", i, vp, vp, sz, P(u64), P(u64))
     sig("swim_topology_generate", i, i, u32, u32, u32, u64, vp)
     sig("swim_sim_generate_view", i, vp, i, u32, u64)
     sig("swim_sim_set_round", i, vp, u32)

@@ -306,6 +306,8 @@ extern "C" int swim_sim_local_range(const swim_sim_t *sim, uint32_t *first, uint
 #include "swim_pushpull.cuh"
 // swim_sim_join: seed joins between steps
 #include "swim_join.cuh"
+// swim_sim_leave: graceful leaves between steps
+#include "swim_leave.cuh"
 // swim_sim_generate_view: the synthetic view graphs generated on the device
 #include "swim_topology.cuh"
 

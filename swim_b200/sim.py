@@ -191,6 +191,17 @@ class Simulator:
                                   C.byref(n), C.byref(f)), "swim_sim_join", self._h)
         return e.value, n.value, f.value
 
+    def leave(self, nodes):
+        """Graceful leaves (DESIGN.md 2.8) at the current round, memberlist's Leave: every listed process that is up goes
+        down as a crash does (and the seeded churn never brings it back), and each member it holds Alive or Suspect that
+        is up receives Dead about it, from it, as an injected datagram. Returns (left, delivered) of this shard. On a
+        sharded handle a collective: every rank is given the same global list."""
+        ids = np.ascontiguousarray(np.atleast_1d(np.asarray(nodes)), dtype=np.uint32)
+        lv, dl = C.c_uint64(), C.c_uint64()
+        check(lib().swim_sim_leave(self._h, ids.ctypes.data, len(ids), C.byref(lv), C.byref(dl)), "swim_sim_leave",
+              self._h)
+        return lv.value, dl.value
+
     def inject(self, events):
         events = np.ascontiguousarray(events, dtype=A.EVENT_DTYPE)
         check(lib().swim_sim_inject(self._h, events.ctypes.data, len(events)), "swim_sim_inject", self._h)

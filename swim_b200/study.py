@@ -10,7 +10,10 @@ Terms, per view entry (observer i, member m) of a live observer:
                `false_dead` = Dead and set after the member's last (re)start — declared dead while it was up;
                `stale_dead_up` = Dead since before the member's last rejoin (the Alive(inc+1) has not arrived).
 The mismatch count of the library (`swim_sim_mismatches`) counts every entry that disagrees with the truth, i.e.
-undetected + suspected + false_dead + stale_dead_up (a Dead entry of a down member agrees, stale or not)."""
+undetected + suspected + false_dead + stale_dead_up (a Dead entry of a down member agrees, stale or not).
+With graceful leaves (Simulator.leave) a down member that left is not a crash: its entries are `left_entries`, split
+into `left_detected` (Dead, set at or after the leave; latency = vlast - leave round) and `left_undetected` (still Alive
+or Suspect), and the mismatch count is undetected + suspected + false_dead + stale_dead_up + left_undetected."""
 import time
 
 import numpy as np
@@ -33,10 +36,12 @@ def event_history(events, n_nodes, upto_round):
     return last_crash, last_rejoin
 
 
-def view_report(sim, events, round_now, max_latency=256):
+def view_report(sim, events, round_now, max_latency=256, left=None):
     """Classify every view entry of this rank's live observers (see the module docstring). Returns a dict of counts
     plus `latency_hist` (index = rounds from crash to the Dead mark, clipped to max_latency). events = None: the crash /
-    rejoin rounds come from the handle's SWIM_ARR_LAST_CRASH / SWIM_ARR_LAST_REJOIN arrays (seeded device-side churn)."""
+    rejoin rounds come from the handle's SWIM_ARR_LAST_CRASH / SWIM_ARR_LAST_REJOIN arrays (seeded device-side churn).
+    left = a bool mask [N] of the processes that left (Simulator.leave): those of them that are down leave the crash
+    categories for left_entries / left_detected / left_undetected, and `leave_latency_hist` is returned as well."""
     cap = sim.cfg.view_cap
     alive = sim.get_array(A.ARR_ALIVE).astype(bool)                  # [N] truth, replicated on every rank
     n_total = alive.shape[0]
@@ -55,6 +60,9 @@ def view_report(sim, events, round_now, max_latency=256):
     member = np.where(occupied, nbr, 0).astype(np.int64)
     m_up = alive[member]
     down = occupied & ~m_up
+    if left is not None:
+        gone = down & np.asarray(left, dtype=bool)[member]
+        down &= ~gone
     up = occupied & m_up
     dead = st == A.DEAD
     crash_at = last_crash[member]
@@ -72,6 +80,14 @@ def view_report(sim, events, round_now, max_latency=256):
         "latency_hist": np.bincount(lat, minlength=max_latency + 1).astype(np.int64),
     }
     out["mismatches"] = out["undetected"] + out["suspected"] + out["false_dead"] + out["stale_dead_up"]
+    if left is not None:  # (a leave marks the leaver's last_crash: the leave round)
+        left_det = gone & dead & (vlast >= crash_at)
+        out["left_entries"] = int(gone.sum())
+        out["left_detected"] = int(left_det.sum())
+        out["left_undetected"] = int((gone & ~dead).sum())
+        out["leave_latency_hist"] = np.bincount(np.clip((vlast - crash_at)[left_det], 0, max_latency),
+                                                minlength=max_latency + 1).astype(np.int64)
+        out["mismatches"] += out["left_undetected"]
     return out
 
 
@@ -109,15 +125,27 @@ def restart_joins(sim, hosts, since, upto):
     return nodes[keep], seeds[keep]
 
 
+def leave_draw(sim, seed, round_, leave_ppm):
+    """The processes that leave gracefully after round `round_`: each up process with probability leave_ppm / 1e6, drawn
+    from a host generator seeded by (seed, round), so every rank, and every suspicion timeout of a sweep, draws the
+    same. Returns the ids (ascending)."""
+    alive = sim.get_array(A.ARR_ALIVE).astype(bool)
+    draw = np.random.default_rng([seed, round_]).random(alive.shape[0]) < leave_ppm * 1e-6
+    return np.flatnonzero(alive & draw).astype(np.uint32)
+
+
 def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None, push_pull_every=0, join_hosts=None,
-                    join_fresh=False):
+                    join_fresh=False, leave_ppm=0):
     """Step `rounds` rounds, sampling the convergence count; returns the time series, the final counters and the final
     view report. `reduce_sum(list_of_numbers) -> list` adds values over ranks (identity for one GPU). push_pull_every = R
     > 0: a push-pull state exchange (Simulator.push_pull; on a sharded handle a collective, which every rank reaches at
     the same round) after every R-th round; its outputs, summed over the calls and the ranks, are in "push_pull".
     join_hosts = the ids of K join hosts: after every step chunk the processes that restarted in it join through all K
     (Simulator.join, `fresh` = join_fresh: the restart lost its state; a collective on a sharded handle). The summed
-    outputs, the joins and the host time of the calls are in "join"."""
+    outputs, the joins and the host time of the calls are in "join". leave_ppm > 0: after every step chunk each up
+    process leaves gracefully (Simulator.leave) with probability leave_ppm / 1e6 (leave_draw, seeded by the config's seed
+    and the round); the report then counts the left members apart, and "leave" holds the calls, ids listed, leavers,
+    records delivered, the host time of the calls and the leave detection latency."""
     red = reduce_sum or (lambda xs: xs)
     series = []
     done = 0
@@ -125,6 +153,9 @@ def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None, push_
     pp = [0, 0, 0]
     jn = [0, 0, 0, 0]  # exchanges, inserted, full, pairs
     join_s = 0.0
+    lv = [0, 0, 0, 0]  # calls, listed, left, delivered
+    leave_s = 0.0
+    left = np.zeros(int(sim.cfg.n_nodes), dtype=bool) if leave_ppm else None
     while done < rounds:
         step = min(sample_every - done % sample_every, rounds - done)
         if push_pull_every:
@@ -139,13 +170,22 @@ def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None, push_
             got = sim.join(nodes, seeds, join_fresh)  # (returns after a device synchronisation)
             join_s += time.perf_counter() - t0
             jn = [a + b for a, b in zip(jn, list(got) + [len(nodes)])]
+        if leave_ppm:
+            ids = leave_draw(sim, int(sim.cfg.seed), int(sim.round), leave_ppm)
+            if len(ids):
+                t0 = time.perf_counter()
+                got = sim.leave(ids)  # (returns after a device synchronisation)
+                leave_s += time.perf_counter() - t0
+                left[ids] = True
+                lv = [a + b for a, b in zip(lv, [1, len(ids)] + list(got))]
         if push_pull_every and done % push_pull_every == 0:
             pp = [a + b for a, b in zip(pp, sim.push_pull())]
         if done % sample_every == 0 or done == rounds:
             series.append((done, int(red([sim.mismatches()])[0])))
     counters = [int(x) for x in red([int(v) for v in sim.counters()])]
-    rep = view_report(sim, events, done)
+    rep = view_report(sim, events, done, left=left)
     hist = np.array(red(rep.pop("latency_hist").tolist()), dtype=np.int64)
+    lhist = np.array(red(rep.pop("leave_latency_hist").tolist()), dtype=np.int64) if left is not None else None
     keys = sorted(rep)
     vals = red([rep[k] for k in keys])
     rep = dict(zip(keys, (int(v) for v in vals)))
@@ -157,4 +197,7 @@ def run_sweep_point(sim, events, rounds, sample_every=10, reduce_sum=None, push_
     if join_hosts is not None and len(join_hosts):
         out["join"] = dict(zip(("exchanges", "inserted", "full"), (int(v) for v in red(jn[:3]))))
         out["join"].update(pairs=jn[3], host_s_rank0=join_s)
+    if leave_ppm:
+        out["leave"] = dict(calls=lv[0], listed=lv[1], left=int(red([lv[2]])[0]), delivered=int(red([lv[3]])[0]),
+                            host_s_rank0=leave_s, leave_latency=latency_stats(lhist))
     return out

@@ -1,0 +1,97 @@
+"""Graceful leaves (swim_sim_leave) on the H100, against the oracle: the shared scenarios at 2^16 nodes for every row
+width, BASELINE config C3 (2^20 nodes, crash burst) with leaves every 25 rounds, and sharded handles of world 2, 3 and 4
+on one device. The emulator versions are in test_emu_leave.py."""
+import numpy as np
+import pytest
+
+import leave_scenarios as S
+from helpers import crash_events, default_config, generate_topology, make_pair
+from leave_oracle import leave as oracle_leave
+from swim_b200 import _abi as A
+
+pytestmark = pytest.mark.gpu
+N16 = 1 << 16
+
+
+@pytest.fixture
+def fused_exchange(monkeypatch):
+    monkeypatch.setenv("SWIM_ROUND_KERNEL", "1")
+
+
+@pytest.mark.parametrize("cap", [32, 64, 128, 256])
+def test_every_row_width(cap):
+    S.leave_every(N16, cap, cap - 8, rounds=18, every=6, seed=cap, loss_ppm=20000, churn_ppm=2000, rejoin_min=2,
+                  rejoin_max=6)
+
+
+@pytest.mark.parametrize("flags,suspicion_max", [(A.F_STRICT_OVERRIDE, 0), (0, 9), (A.F_ROUND_ROBIN, 0)])
+def test_protocol_variants(flags, suspicion_max):
+    S.leave_every(N16, 32, 20, rounds=30, every=5, flags=flags, suspicion_max=suspicion_max, loss_ppm=20000)
+
+
+def test_edge_cases():
+    S.edge_cases()
+
+
+def test_hub():
+    S.hub(N16, 5000)
+
+
+def test_rejoin_after_leave():
+    S.rejoin_after_leave(N16)
+
+
+def test_churn_rejoin_then_leave():
+    S.churn_rejoin_then_leave(4096)
+
+
+def test_save_leave_load():
+    S.save_leave_load(N16)
+
+
+def test_export_after_leave():
+    S.export_after_leave(N16)
+
+
+def test_with_push_pull_and_join():
+    S.with_push_pull_and_join(N16)
+
+
+def test_error_paths():
+    S.error_paths(N16)
+
+
+def test_c3_leaves_every_25_rounds():
+    """C3: N = 1,048,576, D = 32 on 32 slots, 1,048 crashes at round 10; every 25 rounds 0.1 % random nodes leave,
+    together with 30 of the crashed ids (down: ignored), over 200 rounds."""
+    n = 1 << 20
+    cfg = default_config(n_nodes=n, seed=0x5EED0001 + 3)
+    rng = np.random.default_rng(3)
+    crashed = np.sort(rng.choice(n, size=n // 1000, replace=False)).astype(np.uint32)
+    sim, orc = make_pair(cfg, generate_topology("random", n, 32, 32, seed=3))
+    ev = crash_events(10, crashed)
+    sim.inject(ev)
+    orc.inject(ev)
+    for _ in range(8):
+        sim.step(25)
+        orc.step(25)
+        ids = np.concatenate([rng.choice(n, size=n // 1000, replace=False).astype(np.uint32), crashed[:30]])
+        got = sim.leave(ids)
+        assert got == oracle_leave(orc, ids) and got[1] > 0, got
+        assert sim.digest() == orc.digest(), f"digest differs at round {sim.round}"
+        assert sim.counters().tolist() == orc.counters().tolist()
+        assert sim.mismatches() == orc.mismatches()
+    sim.step(5)
+    orc.step(5)
+    assert sim.digest() == orc.digest() and sim.mismatches() == orc.mismatches()
+    sim.close()
+
+
+@pytest.mark.usefixtures("fused_exchange")
+@pytest.mark.parametrize("world", [2, 3, 4])
+def test_sharded(world):
+    S.sharded_leaves(world, 1100, "p2p", devices=[0] * world, rounds=36, every=12)
+
+
+def test_sharded_equals_single_shard():
+    S.sharded_equals_single_shard(1 << 18, 4, [0] * 4)
