@@ -1,5 +1,5 @@
 // swim_join.cuh — seed joins between steps (DESIGN.md §2.7), on the device. Compiled as part of swim_sim.cu's
-// translation unit, after swim_pushpull.cuh (whose snapshot, gather and merge it uses).
+// translation unit, after swim_pushpull.cuh (whose merge, scan and call skeleton it uses).
 //
 // memberlist's Join(joinHosts): each pair (joiner j, seed s) is one full-state exchange between j and s, whether or not
 // either lists the other. The exchange is push-pull's: both states are read from a snapshot, and each receiver merges
@@ -105,9 +105,7 @@ int join_local(swim_sim *sim, Scratch &s, const uint2 *pr, uint32_t np, const Pp
   ++sim->launches;
   GRAPH_TRY(sim, cudaGetLastError());
   int rc;
-  if ((rc = scan_u32(sim, s, cnt, n, seg))) return rc;
-  GRAPH_TRY(sim, cudaMemcpyAsync(&E, seg + n, 8, cudaMemcpyDeviceToHost, sim->stream));
-  GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
+  if ((rc = scan_total(sim, s, cnt, n, seg, &E))) return rc;
   if (E) {
     // (receiver, sender) order: a stable sort of the directions by sender, then a stable sort of that by receiver
     const uint32_t *k1, *v1, *k2, *v2;
@@ -122,38 +120,11 @@ int join_local(swim_sim *sim, Scratch &s, const uint2 *pr, uint32_t np, const Pp
     SWIM_LAUNCH(join_take_kernel, g, kGT, sim->stream, v2, k1, (size_t)E, chooser);
     ++sim->launches;
     GRAPH_TRY(sim, cudaGetLastError());
-    PpSnap snap;
-    if (gsnap) snap = *gsnap;
-    else if ((rc = pp_snapshot(sim, s, &snap))) return rc;
-    if ((rc = pp_merge(sim, snap, part, seg, chooser, res))) return rc;
+    if ((rc = pp_merge(sim, s, gsnap, part, seg, chooser, res))) return rc;
   }
   GRAPH_TRY(sim, cudaMemcpyAsync(h, res, 3 * sizeof(u64), cudaMemcpyDeviceToHost, sim->stream));
   GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
   return SWIM_OK;
-}
-
-// The whole call on one rank. Sharded, a collective: barrier (every rank's earlier calls are done), the fresh resets of
-// this rank's joiners, barrier (every reset is done before anyone copies a row), the gather of the global snapshot,
-// barrier, the merge into this rank's receivers, and a last barrier that sums inserts + vacated slots, so that every rank
-// marks the view changed exactly when some rank changed a membership. The scratch is freed before that barrier (see
-// push_pull_sharded). *edited = that sum (single shard: this shard's).
-int join_run(swim_sim *sim, const swim_join_t *joins, uint32_t np, bool fresh, u64 h[3], u64 *edited) {
-  const bool sharded = sim->dev.world > 1;
-  u64 vacated = 0;
-  int rc;
-  {
-    Scratch s(sim);
-    uint2 *pr;
-    PpSnap snap;
-    SCRATCH(s, pr, np);
-    GRAPH_TRY(sim, cudaMemcpyAsync(pr, joins, (size_t)np * sizeof(uint2), cudaMemcpyHostToDevice, sim->stream));
-    if (sharded && ((rc = pp_gather_alloc(sim, s, &snap)) || (rc = coll_barrier(sim)))) return rc;
-    if (fresh && (rc = join_reset(sim, s, pr, np, &vacated))) return rc;
-    if (sharded && ((rc = coll_barrier(sim)) || (rc = pp_gather(sim, snap)) || (rc = coll_barrier(sim)))) return rc;
-    if ((rc = join_local(sim, s, pr, np, sharded ? &snap : nullptr, h))) return rc;
-  }
-  if (!sharded) { *edited = h[0] + vacated; return SWIM_OK; }
-  return coll_barrier(sim, h[0] + vacated, edited);
 }
 
 } // namespace
@@ -161,13 +132,9 @@ int join_run(swim_sim *sim, const swim_join_t *joins, uint32_t np, bool fresh, u
 extern "C" int swim_sim_join(swim_sim_t *sim, const swim_join_t *joins, size_t n, uint32_t flags, uint64_t *n_exchanges,
                              uint64_t *n_inserted, uint64_t *n_full) {
   if (!sim || (!joins && n)) return SWIM_EINVAL;
+  int rc;
+  if ((rc = between_steps_check(sim, "swim_sim_join"))) return rc;
   const SimDev &d = sim->dev;
-  if (d.world != 1 && !sim->connected) {
-    set_error(sim, "swim_sim_join: world > 1 needs swim_sim_ipc_connect or swim_sim_connect (every rank makes the call)");
-    return SWIM_ESTATE;
-  }
-  if (!sim->view_set) { set_error(sim, "swim_sim_join: no view installed"); return SWIM_ESTATE; }
-  if (sim->failed) { set_error(sim, "swim_sim_join: an earlier step failed part-way; the handle's device state is undefined"); return SWIM_ESTATE; }
   if (flags & ~(uint32_t)SWIM_JOIN_FRESH) { set_error(sim, "swim_sim_join: unknown flags 0x%x", flags); return SWIM_EINVAL; }
   if (n > 0x7FFFFFFFull) { set_error(sim, "swim_sim_join: %zu pairs in one call (at most 2^31 - 1)", n); return SWIM_EINVAL; }
   for (size_t x = 0; x < n; ++x)
@@ -176,16 +143,23 @@ extern "C" int swim_sim_join(swim_sim_t *sim, const swim_join_t *joins, size_t n
                 joins[x].seed);
       return SWIM_EINVAL;
     }
-  u64 h[3] = {0, 0, 0}, edited = 0;
+  u64 h[3] = {0, 0, 0}, vacated = 0;
   if (n) {
-    cudaSetDevice(sim->device);
-    const int rc = join_run(sim, joins, (uint32_t)n, (flags & SWIM_JOIN_FRESH) != 0, h, &edited);
-    if (rc) {
-      if (d.world != 1) sim->failed = true; // the ranks are no longer in step
-      return rc;
-    }
-    if (edited) mark_edited(sim); // members were inserted or removed: the mail graph is rebuilt by the next step
-    else sim->tdead_dirty = true;
+    const uint32_t np = (uint32_t)n;
+    uint2 *pr = nullptr;
+    rc = between_steps(
+        sim,
+        [&](Scratch &s, const PpSnap *gsnap, u64 *edited) { // members inserted or removed
+          const int rc = join_local(sim, s, pr, np, gsnap, h);
+          *edited = h[0] + vacated;
+          return rc;
+        },
+        [&](Scratch &s) -> int { // the upload, and SWIM_JOIN_FRESH's resets
+          SCRATCH(s, pr, np);
+          GRAPH_TRY(sim, cudaMemcpyAsync(pr, joins, (size_t)np * sizeof(uint2), cudaMemcpyHostToDevice, sim->stream));
+          return flags & SWIM_JOIN_FRESH ? join_reset(sim, s, pr, np, &vacated) : SWIM_OK;
+        });
+    if (rc) return rc;
   }
   if (n_exchanges) *n_exchanges = h[2];
   if (n_inserted) *n_inserted = h[0];

@@ -1,5 +1,5 @@
 // swim_leave.cuh — graceful leaves between steps (DESIGN.md §2.8), on the device. Compiled as part of swim_sim.cu's
-// translation unit, after swim_join.cuh (whose scratch, scan, sort and gather helpers it uses).
+// translation unit, after swim_join.cuh (whose scratch, scan and sort helpers and call skeleton it uses).
 //
 // memberlist's Leave: the departing process broadcasts Dead about itself (From = itself) and waits for the gossip to
 // spread before it stops. Here the wait is condensed into the call: every leaver goes down as a CRASH at the current
@@ -104,9 +104,7 @@ int leave_local(swim_sim *sim, Scratch &s, const uint32_t *ids, uint32_t np, con
   ++sim->launches;
   GRAPH_TRY(sim, cudaGetLastError());
   int rc;
-  if ((rc = scan_u32(sim, s, mark, N, pos))) return rc;
-  GRAPH_TRY(sim, cudaMemcpyAsync(&nl, pos + N, 8, cudaMemcpyDeviceToHost, sim->stream));
-  GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
+  if ((rc = scan_total(sim, s, mark, N, pos, &nl))) return rc;
   if (nl) {
     uint32_t *lv, *key;
     SCRATCH(s, lv, nl);
@@ -117,9 +115,7 @@ int leave_local(swim_sim *sim, Scratch &s, const uint32_t *ids, uint32_t np, con
                 gsnap ? gsnap->nbr : (const uint32_t *)d.nbr, gsnap ? gsnap->vst : (const uint8_t *)d.vst, cnt, key);
     sim->launches += 2;
     GRAPH_TRY(sim, cudaGetLastError());
-    if ((rc = scan_u32(sim, s, cnt, n, seg))) return rc;
-    GRAPH_TRY(sim, cudaMemcpyAsync(&E, seg + n, 8, cudaMemcpyDeviceToHost, sim->stream));
-    GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
+    if ((rc = scan_total(sim, s, cnt, n, seg, &E))) return rc;
     if (E) {
       const uint32_t *rcv, *who;
       DevEvent *ev;
@@ -140,50 +136,26 @@ int leave_local(swim_sim *sim, Scratch &s, const uint32_t *ids, uint32_t np, con
   return SWIM_OK;
 }
 
-// Sharded, a collective: barrier (every rank's earlier calls are done), the gather of the global snapshot, barrier (no
-// rank writes a row or alive[] before every rank has its copy), then on every rank the departure of every leaver in its
-// replicated arrays and the merge into its own recipients, the scratch freed, and a last barrier (see push_pull_sharded:
-// a peer on this device may start its round kernels right after it).
-int leave_run(swim_sim *sim, const uint32_t *nodes, uint32_t np, u64 h[2]) {
-  const bool sharded = sim->dev.world > 1;
-  int rc;
-  {
-    Scratch s(sim);
-    uint32_t *ids;
-    PpSnap snap;
-    SCRATCH(s, ids, np);
-    GRAPH_TRY(sim, cudaMemcpyAsync(ids, nodes, (size_t)np * 4, cudaMemcpyHostToDevice, sim->stream));
-    if (sharded && ((rc = pp_gather_alloc(sim, s, &snap)) || (rc = coll_barrier(sim)) || (rc = pp_gather(sim, snap)) ||
-                    (rc = coll_barrier(sim))))
-      return rc;
-    if ((rc = leave_local(sim, s, ids, np, sharded ? &snap : nullptr, h))) return rc;
-  }
-  return sharded ? coll_barrier(sim) : SWIM_OK;
-}
-
 } // namespace
 
 extern "C" int swim_sim_leave(swim_sim_t *sim, const uint32_t *nodes, size_t n, uint64_t *n_left, uint64_t *n_delivered) {
   if (!sim || (!nodes && n)) return SWIM_EINVAL;
+  int rc;
+  if ((rc = between_steps_check(sim, "swim_sim_leave"))) return rc;
   const SimDev &d = sim->dev;
-  if (d.world != 1 && !sim->connected) {
-    set_error(sim, "swim_sim_leave: world > 1 needs swim_sim_ipc_connect or swim_sim_connect (every rank makes the call)");
-    return SWIM_ESTATE;
-  }
-  if (!sim->view_set) { set_error(sim, "swim_sim_leave: no view installed"); return SWIM_ESTATE; }
-  if (sim->failed) { set_error(sim, "swim_sim_leave: an earlier step failed part-way; the handle's device state is undefined"); return SWIM_ESTATE; }
   if (n > 0x7FFFFFFFull) { set_error(sim, "swim_sim_leave: %zu ids in one call (at most 2^31 - 1)", n); return SWIM_EINVAL; }
   for (size_t x = 0; x < n; ++x)
     if (nodes[x] >= d.N) { set_error(sim, "swim_sim_leave: id %zu (%u) >= N = %u", x, nodes[x], d.N); return SWIM_EINVAL; }
   u64 h[2] = {0, 0};
-  if (n) {
-    cudaSetDevice(sim->device);
-    const int rc = leave_run(sim, nodes, (uint32_t)n, h);
-    if (rc) {
-      if (d.world != 1) sim->failed = true; // the ranks are no longer in step
-      return rc;
-    }
-    sim->tdead_dirty = true; // alive[] and rows changed: the crashed-member bitmaps and per-node records are re-derived
+  if (n) { // no membership changes (edited stays 0): alive[] and rows changed, so only the per-node state is re-derived
+    const uint32_t np = (uint32_t)n;
+    rc = between_steps(sim, [&](Scratch &s, const PpSnap *gsnap, u64 *) -> int {
+      uint32_t *ids;
+      SCRATCH(s, ids, np);
+      GRAPH_TRY(sim, cudaMemcpyAsync(ids, nodes, (size_t)np * 4, cudaMemcpyHostToDevice, sim->stream));
+      return leave_local(sim, s, ids, np, gsnap, h);
+    });
+    if (rc) return rc;
   }
   if (n_left) *n_left = h[0];
   if (n_delivered) *n_delivered = h[1];

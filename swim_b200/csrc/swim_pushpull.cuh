@@ -11,6 +11,9 @@
 // alive[] and the round, so all ranks agree without exchanging them), and each rank merges into its own receivers.
 #pragma once
 
+#include <cstddef>
+#include <type_traits>
+
 #include "swim_graph.cuh"
 
 namespace {
@@ -160,27 +163,36 @@ __global__ void __launch_bounds__(kThreads) push_pull_kernel(SimDev d, uint32_t 
 } // namespace
 
 namespace {
-// The snapshot of a single shard: copies of its rows and incarnations, taken on the stream before any row changes.
-int pp_snapshot(swim_sim *sim, Scratch &s, PpSnap *snap) {
+// A snapshot of `rows` rows by global id and their incarnations, in scratch: on a single shard (`copy`) copies of its
+// rows taken on the stream before any row changes, sharded the buffers that every rank's rows are gathered into.
+int pp_snapshot(swim_sim *sim, Scratch &s, size_t rows, bool copy, PpSnap *snap) {
   const SimDev &d = sim->dev;
-  const size_t n = d.n, slots = n * d.cap;
+  const size_t slots = rows * d.cap;
   uint32_t *nb, *vi, *si;
   uint8_t *vs;
   SCRATCH(s, nb, slots);
   SCRATCH(s, vi, slots);
-  SCRATCH(s, si, n);
+  SCRATCH(s, si, rows);
   SCRATCH(s, vs, slots);
-  GRAPH_TRY(sim, cudaMemcpyAsync(nb, d.nbr, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
-  GRAPH_TRY(sim, cudaMemcpyAsync(vi, d.vinc, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
-  GRAPH_TRY(sim, cudaMemcpyAsync(si, d.self_inc, n * 4, cudaMemcpyDeviceToDevice, sim->stream));
-  GRAPH_TRY(sim, cudaMemcpyAsync(vs, d.vst, slots, cudaMemcpyDeviceToDevice, sim->stream));
+  if (copy) {
+    GRAPH_TRY(sim, cudaMemcpyAsync(nb, d.nbr, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
+    GRAPH_TRY(sim, cudaMemcpyAsync(vi, d.vinc, slots * 4, cudaMemcpyDeviceToDevice, sim->stream));
+    GRAPH_TRY(sim, cudaMemcpyAsync(si, d.self_inc, rows * 4, cudaMemcpyDeviceToDevice, sim->stream));
+    GRAPH_TRY(sim, cudaMemcpyAsync(vs, d.vst, slots, cudaMemcpyDeviceToDevice, sim->stream));
+  }
   snap->nbr = nb; snap->vinc = vi; snap->self_inc = si; snap->vst = vs;
   return SWIM_OK;
 }
 
-// push_pull_kernel at the handle's row width: every local receiver j merges {part[j]} and chooser[seg[j] .. seg[j + 1]).
-int pp_merge(swim_sim *sim, const PpSnap &snap, const uint32_t *part, const u64 *seg, const uint32_t *chooser, u64 *res) {
+// push_pull_kernel at the handle's row width: every local receiver j merges {part[j]} and chooser[seg[j] .. seg[j + 1]),
+// from `gsnap` (sharded: the gathered global snapshot) or, on a single shard, from a snapshot of its rows taken here.
+int pp_merge(swim_sim *sim, Scratch &s, const PpSnap *gsnap, const uint32_t *part, const u64 *seg, const uint32_t *chooser,
+             u64 *res) {
   const SimDev &d = sim->dev;
+  PpSnap snap;
+  int rc;
+  if (gsnap) snap = *gsnap;
+  else if ((rc = pp_snapshot(sim, s, d.n, true, &snap))) return rc;
   const int g = grid_of(sim, (d.n + kWarpsPerBlock - 1) / kWarpsPerBlock);
   switch (d.cap / 32) {
     case 1: SWIM_LAUNCH(push_pull_kernel<1>, g, kThreads, sim->stream, d, sim->round, snap, part, seg, chooser, res); break;
@@ -193,8 +205,18 @@ int pp_merge(swim_sim *sim, const PpSnap &snap, const uint32_t *part, const u64 
   return SWIM_OK;
 }
 
-// The exchange on this shard's receivers. Sharded: between the gather barriers of swim_sim_push_pull, with `snap` the
-// gathered global snapshot. h = {inserted, dropped on a full row, exchanges} of this shard.
+// Counts to positions: out[0..n] = the exclusive scan of in[0..n), and *total = out[n] on the host (the stream is
+// synchronised, so device-to-host copies queued before this call have landed too).
+int scan_total(swim_sim *sim, Scratch &s, const uint32_t *in, size_t n, u64 *out, u64 *total) {
+  int rc;
+  if ((rc = scan_u32(sim, s, in, n, out))) return rc;
+  GRAPH_TRY(sim, cudaMemcpyAsync(total, out + n, 8, cudaMemcpyDeviceToHost, sim->stream));
+  GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
+  return SWIM_OK;
+}
+
+// The exchange on this shard's receivers. Sharded: `gsnap` is the gathered global snapshot. h = {inserted, dropped on a
+// full row, exchanges} of this shard.
 int push_pull_local(swim_sim *sim, Scratch &s, const PpSnap *gsnap, u64 h[3]) {
   const SimDev &d = sim->dev;
   const size_t n = d.n;
@@ -214,90 +236,88 @@ int push_pull_local(swim_sim *sim, Scratch &s, const PpSnap *gsnap, u64 h[3]) {
               cnt, res + 2);
   ++sim->launches;
   GRAPH_TRY(sim, cudaGetLastError());
-  int rc;
-  if ((rc = scan_u32(sim, s, cnt, n, seg))) return rc;
-  GRAPH_TRY(sim, cudaMemcpyAsync(&E, seg + n, 8, cudaMemcpyDeviceToHost, sim->stream));
   GRAPH_TRY(sim, cudaMemcpyAsync(&ex, res + 2, 8, cudaMemcpyDeviceToHost, sim->stream));
-  GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
+  int rc;
+  if ((rc = scan_total(sim, s, cnt, n, seg, &E))) return rc;
   if (E || ex) { // (sharded, a shard's nodes may pull from partners elsewhere while none of its own is chosen)
     // the choosers of every local node, ascending: a stable sort of the partner array by partner
     const uint32_t *skey, *chooser = nullptr;
     if (E && (rc = sort_by_key(sim, s, key ? key : part, rows, 1, E, d.N, &skey, &chooser))) return rc;
-    PpSnap snap;
-    if (gsnap) snap = *gsnap;
-    else if ((rc = pp_snapshot(sim, s, &snap))) return rc;
-    if ((rc = pp_merge(sim, snap, part, seg, chooser, res))) return rc;
+    if ((rc = pp_merge(sim, s, gsnap, part, seg, chooser, res))) return rc;
   }
   GRAPH_TRY(sim, cudaMemcpyAsync(h, res, 3 * sizeof(u64), cudaMemcpyDeviceToHost, sim->stream));
   GRAPH_TRY(sim, cudaStreamSynchronize(sim->stream));
   return SWIM_OK;
 }
 
-// Sharded: device buffers for the global snapshot, [world * per] rows addressed by global id ...
-int pp_gather_alloc(swim_sim *sim, Scratch &s, PpSnap *snap) {
+// The entry check of the collective calls between steps (push-pull, joins, leaves), in this order: a sharded handle
+// must be connected to its peers, a view installed, and no earlier step failed part-way.
+int between_steps_check(swim_sim *sim, const char *api) {
+  if (sim->dev.world != 1 && !sim->connected) {
+    set_error(sim, "%s: world > 1 needs swim_sim_ipc_connect or swim_sim_connect (every rank makes the call)", api);
+    return SWIM_ESTATE;
+  }
+  if (!sim->view_set) { set_error(sim, "%s: no view installed", api); return SWIM_ESTATE; }
+  if (sim->failed) { set_error(sim, "%s: an earlier step failed part-way; the handle's device state is undefined", api); return SWIM_ESTATE; }
+  return SWIM_OK;
+}
+
+// The body of a call between steps on one rank: `pre(s)` (optional), then `local(s, gsnap, &edited)` on this shard's
+// nodes, with gsnap = null on a single shard (the call reads this shard's rows). Sharded, a collective: barrier (every
+// rank's earlier calls are done); `pre` and a barrier (every rank's is done before anyone copies a row); the gather of
+// the global snapshot into gsnap; barrier (nobody changes a row or alive[] before every rank has its copy); `local`; and
+// a last barrier that sums `edited`, so that every rank marks the view changed, and rebuilds at the next step, exactly
+// when some rank changed a membership. The scratch is freed before that barrier: a peer that shares this device may
+// start its round kernels right after it, and cudaFree would wait for them while they wait for this rank.
+template <typename Local, typename Pre>
+int between_steps_body(swim_sim *sim, Local &local, Pre &pre, u64 *edited) {
   const SimDev &d = sim->dev;
-  const size_t rows = (size_t)d.world * d.per, gslots = rows * d.cap;
-  uint32_t *nb, *vi, *si;
-  uint8_t *vs;
-  SCRATCH(s, nb, gslots);
-  SCRATCH(s, vi, gslots);
-  SCRATCH(s, si, rows);
-  SCRATCH(s, vs, gslots);
-  snap->nbr = nb; snap->vinc = vi; snap->self_inc = si; snap->vst = vs;
-  return SWIM_OK;
-}
-
-// ... and every rank's rows and incarnations gathered into them (between barriers: no rank changes a row meanwhile).
-int pp_gather(swim_sim *sim, const PpSnap &snap) {
-  int rc;
-  if ((rc = coll_gather(sim, kCollNbr, (void *)snap.nbr)) || (rc = coll_gather(sim, kCollVst, (void *)snap.vst)) ||
-      (rc = coll_gather(sim, kCollVinc, (void *)snap.vinc)) || (rc = coll_gather(sim, kCollSelfInc, (void *)snap.self_inc)))
-    return rc;
-  return SWIM_OK;
-}
-
-// Sharded: barrier (every rank's earlier calls are done), gather the global snapshot, barrier (nobody changes a row
-// before every rank has its copy), the local exchange, and a last barrier that sums the inserts, so that every rank
-// marks the view changed — and rebuilds at the next step — exactly when some rank inserted. The scratch is freed before
-// that barrier: a peer that shares this device may start its round kernels right after it, and cudaFree would wait for
-// them while they wait for this rank.
-int push_pull_sharded(swim_sim *sim, u64 h[3], u64 *inserted_all) {
+  const bool sharded = d.world > 1;
   int rc;
   {
     Scratch s(sim);
     PpSnap snap;
-    if ((rc = pp_gather_alloc(sim, s, &snap))) return rc;
-    if ((rc = coll_barrier(sim))) return rc;
-    if ((rc = pp_gather(sim, snap))) return rc;
-    if ((rc = coll_barrier(sim))) return rc;
-    if ((rc = push_pull_local(sim, s, &snap, h))) return rc;
+    if (sharded && ((rc = pp_snapshot(sim, s, (size_t)d.world * d.per, false, &snap)) || (rc = coll_barrier(sim)))) return rc;
+    if constexpr (!std::is_same<Pre, std::nullptr_t>::value)
+      if ((rc = pre(s)) || (sharded && (rc = coll_barrier(sim)))) return rc;
+    if (sharded && ((rc = coll_gather(sim, kCollNbr, (void *)snap.nbr)) || (rc = coll_gather(sim, kCollVst, (void *)snap.vst)) ||
+                    (rc = coll_gather(sim, kCollVinc, (void *)snap.vinc)) ||
+                    (rc = coll_gather(sim, kCollSelfInc, (void *)snap.self_inc)) || (rc = coll_barrier(sim))))
+      return rc;
+    if ((rc = local(s, sharded ? &snap : nullptr, edited))) return rc;
   }
-  return coll_barrier(sim, h[0], inserted_all);
+  return sharded ? coll_barrier(sim, *edited, edited) : SWIM_OK;
+}
+
+// A call between steps, body and ending: after an error a sharded handle is failed (the ranks are no longer in step);
+// otherwise the mail graph is rebuilt by the next step if memberships changed, and in any case the crashed-member
+// bitmaps and per-node records are re-derived before the next round.
+template <typename Local, typename Pre = std::nullptr_t>
+int between_steps(swim_sim *sim, Local local, Pre pre = nullptr) {
+  cudaSetDevice(sim->device);
+  u64 edited = 0;
+  const int rc = between_steps_body(sim, local, pre, &edited);
+  if (rc) {
+    if (sim->dev.world != 1) sim->failed = true;
+    return rc;
+  }
+  if (edited) mark_edited(sim);
+  else sim->tdead_dirty = true;
+  return SWIM_OK;
 }
 } // namespace
 
 extern "C" int swim_sim_push_pull(swim_sim_t *sim, uint64_t *n_exchanges, uint64_t *n_inserted, uint64_t *n_full) {
   if (!sim) return SWIM_EINVAL;
-  const SimDev &d = sim->dev;
-  if (d.world != 1 && !sim->connected) {
-    set_error(sim, "swim_sim_push_pull: world > 1 needs swim_sim_ipc_connect or swim_sim_connect (every rank makes the call)");
-    return SWIM_ESTATE;
-  }
-  if (!sim->view_set) { set_error(sim, "swim_sim_push_pull: no view installed"); return SWIM_ESTATE; }
-  if (sim->failed) { set_error(sim, "swim_sim_push_pull: an earlier step failed part-way; the handle's device state is undefined"); return SWIM_ESTATE; }
-  cudaSetDevice(sim->device);
-  u64 h[3] = {0, 0, 0}, ins = 0;
-  if (d.world == 1) {
-    Scratch s(sim);
-    int rc = push_pull_local(sim, s, nullptr, h);
-    if (rc) return rc;
-    ins = h[0];
-  } else {
-    int rc = push_pull_sharded(sim, h, &ins);
-    if (rc) { sim->failed = true; return rc; } // the ranks are no longer in step
-  }
-  if (ins) mark_edited(sim); // members were inserted: the mail graph is rebuilt by the next step
-  else sim->tdead_dirty = true;
+  int rc;
+  if ((rc = between_steps_check(sim, "swim_sim_push_pull"))) return rc;
+  u64 h[3] = {0, 0, 0};
+  rc = between_steps(sim, [&](Scratch &s, const PpSnap *gsnap, u64 *edited) {
+    const int rc = push_pull_local(sim, s, gsnap, h);
+    *edited = h[0];
+    return rc;
+  });
+  if (rc) return rc;
   if (n_exchanges) *n_exchanges = h[2];
   if (n_inserted) *n_inserted = h[0];
   if (n_full) *n_full = h[1];

@@ -1,34 +1,19 @@
 """Scenarios of the seed joins between steps (swim_sim_join, DESIGN.md 2.7), shared by the emulator tests (small sizes)
 and the H100 tests (2^16 nodes and up). Every call is checked against the CPU oracle's statement
-(tests/join_oracle.c, oracle_join): the three outputs, every state array, the counters and the digest. The sharded
-scenarios hold the shards' sums to the single-shard oracle, as sharded_edit_scenarios does."""
+(tests/between_steps_oracle.c, oracle_join): the three outputs, every state array, the counters and the digest. The
+sharded scenarios hold the shards' sums to the single-shard oracle (between_steps_scenarios)."""
+from functools import partial
+
 import numpy as np
 import pytest
 
-from helpers import assert_same_state, crash_events, default_config, generate_topology, make_pair, random_events
-from join_oracle import join as oracle_join
-from push_pull_oracle import push_pull as oracle_push_pull
+import between_steps_scenarios as B
+from between_steps_oracle import join as oracle_join, push_pull as oracle_push_pull
+from between_steps_scenarios import pair, step
+from helpers import assert_same_state, crash_events, random_events
 from swim_b200 import _abi as A
 
-
-def join(sim, orc, nodes, seeds, fresh=False, where=""):
-    got, want = sim.join(nodes, seeds, fresh), oracle_join(orc, nodes, seeds, fresh)
-    assert got == want, (where, got, want)
-    assert_same_state(sim, orc, f"after join, {where}")
-    return got
-
-
-def step(sim, orc, rounds, check=True):
-    sim.step(rounds)
-    orc.step(rounds)
-    if check:
-        assert_same_state(sim, orc, f"round {sim.round}")
-
-
-def pair(n, cap=32, deg=32, kind="random", seed=1, **kw):
-    kw.setdefault("suspicion_rounds", 3)
-    cfg = default_config(n_nodes=n, view_cap=cap, seed=seed, **kw)
-    return make_pair(cfg, generate_topology(kind, n, cap, deg, seed=seed))
+join = partial(B.call, "join")
 
 
 def restart_pairs(rng, n, hosts, frac=0.05):
@@ -213,85 +198,25 @@ def with_push_pull(n, cap=32, deg=12, seed=10):
 
 
 def error_paths(n=40):
-    """SWIM_EINVAL on an id >= N or node == seed, before anything changes; SWIM_ESTATE on a sharded handle that is not
-    connected and before a view is installed."""
-    from swim_b200._lib import SwimError
-    from swim_b200.sim import Simulator
-    sim, orc = pair(n, 32, 10, seed=11)
-    before = sim.state()
-    for nodes, seeds in (([1, 2], [3, n]), ([n, 2], [3, 4]), ([1, 2], [3, 2])):
-        with pytest.raises(SwimError) as e:
-            sim.join(nodes, seeds, fresh=True)
-        assert e.value.code == A.EINVAL
-    after = sim.state()
-    assert all(np.array_equal(before[k], after[k]) for k in before)
-    sim.close()
-    shard = Simulator(default_config(n_nodes=n, world=2, rank=0))
-    shard.set_view(generate_topology("random", n, 32, 16, seed=12))
-    bare = Simulator(default_config(n_nodes=n))
-    for s in (shard, bare):
-        with pytest.raises(SwimError) as e:
-            s.join([1], [2])
-        assert e.value.code == A.ESTATE
-        s.close()
+    """SWIM_EINVAL on an id >= N or node == seed."""
+    B.error_paths("join", ([1], [2]), [(nodes, seeds, True) for nodes, seeds in (([1, 2], [3, n]), ([n, 2], [3, 4]),
+                                                                                ([1, 2], [3, 2]))], n)
+
+
+sharded_not_connected = partial(B.sharded_not_connected, "join", ([30], [1], True))
 
 
 # ------------------------------------------------------------------ sharded handles
 def sharded_joins(world, n, mode, devices=None, rounds=24, every=6):
-    """Joins through 3 seeds every `every` rounds on `world` ranks, alternately fresh and not, under events and loss;
-    the shards' sums against the single-shard oracle after every call and every chunk."""
-    import sharded_edit_scenarios as SE
-    sh, orc = SE.setup(world, n, 14, mode, seed=13, devices=devices, rounds=rounds, loss_ppm=10000)
+    """Joins through 3 seeds every `every` rounds on `world` ranks, alternately fresh and not, under events and loss."""
     rng = np.random.default_rng(13)
     hosts = rng.choice(n, size=3, replace=False)
-    tot = np.zeros(3, dtype=np.int64)
-    for k in range(rounds // every):
-        SE.step(sh, orc, [every])
-        nodes, seeds = restart_pairs(rng, n, hosts)
-        fresh = k % 2 == 1
-        got, want = sh.total(lambda s: s.join(nodes, seeds, fresh)), oracle_join(orc, nodes, seeds, fresh)
-        assert got == want, (k, got, want)
-        sh.check(orc, f"after join {k}")
-        tot += got
-    SE.step(sh, orc, [1, 3])
-    assert tot[0] > 0 and tot[1] > 0, tot
-    sh.close()
+    B.sharded_every("join", lambda k: (*restart_pairs(rng, n, hosts), k % 2 == 1), world, n, mode, devices, rounds,
+                    every)
 
 
 def sharded_equals_single_shard(n, world, devices, mode="p2p"):
-    """No rounds: at n nodes a fresh join of 1 % of the nodes through 3 seeds, then a plain one, on the shards and on the
-    single-shard handle, give the same arrays and totals."""
-    import sharded_edit_scenarios as SE
-    from swim_b200.sim import Simulator
-    kw = SE.config(n, 14, suspicion_rounds=4)
-    nbr = generate_topology("random", n, 32, 16, seed=14)
-    sh = SE.Shards(world, kw, nbr, mode, devices)
-    one = Simulator(default_config(device=devices[0] if devices else -1, **kw))
-    one.set_view(nbr)
-    rng = np.random.default_rng(14)
-    alive = (rng.random(n) > 0.05).astype(np.uint8)
-    one.set_array(A.ARR_ALIVE, alive)
-    for s in sh.sims:
-        s.set_array(A.ARR_ALIVE, alive)
-    for fresh in (True, False):
-        nodes, seeds = restart_pairs(rng, n, rng.choice(n, size=3, replace=False), 0.01)
-        want = one.join(nodes, seeds, fresh)
-        assert sh.total(lambda s: s.join(nodes, seeds, fresh)) == want and want[1] > 0, want
-        for a in range(A.ARR_COUNT):
-            assert np.array_equal(sh.array(a), one.get_array(a)), (fresh, A.ARRAY_NAMES[a])
-    sh.close()
-    one.close()
-
-
-def sharded_not_connected(n=40):
-    from swim_b200._lib import SwimError
-    from swim_b200.sim import Simulator
-    shard = Simulator(default_config(n_nodes=n, world=2, rank=1))
-    shard.set_view(generate_topology("random", n, 32, 16, seed=12))
-    before = shard.state()
-    with pytest.raises(SwimError) as e:
-        shard.join([30], [1], fresh=True)
-    assert e.value.code == A.ESTATE
-    after = shard.state()
-    assert all(np.array_equal(before[k], after[k]) for k in before)
-    shard.close()
+    """A fresh join of 1 % of the nodes through 3 seeds, then a plain one."""
+    B.sharded_equals_single_shard(
+        "join", lambda rng, k: (*restart_pairs(rng, n, rng.choice(n, size=3, replace=False), 0.01), k == 0), n, world,
+        devices, mode)

@@ -1,36 +1,19 @@
 """Scenarios of the graceful leaves between steps (swim_sim_leave, DESIGN.md 2.8), shared by the emulator tests (small
 sizes) and the H100 tests (2^16 nodes and up). Every call is checked against the CPU oracle's statement
-(tests/leave_oracle.c, oracle_leave): both outputs, every state array, the counters, the digest and the mismatch count,
-right after the call and after further steps. The sharded scenarios hold the shards' sums to the single-shard oracle, as
-sharded_edit_scenarios does."""
-import numpy as np
-import pytest
+(tests/between_steps_oracle.c, oracle_leave): both outputs, every state array, the counters, the digest and the mismatch
+count, right after the call and after further steps. The sharded scenarios hold the shards' sums to the single-shard
+oracle (between_steps_scenarios)."""
+from functools import partial
 
-from helpers import assert_same_state, crash_events, default_config, generate_topology, make_events, make_pair, random_events
-from leave_oracle import leave as oracle_leave
+import numpy as np
+
+import between_steps_scenarios as B
+from between_steps_scenarios import pair, step
+from helpers import assert_same_state, crash_events, generate_topology, make_events, random_events
 from swim_b200 import _abi as A
 
 NM = A.NO_MEMBER
-
-
-def leave(sim, orc, nodes, where=""):
-    got, want = sim.leave(nodes), oracle_leave(orc, nodes)
-    assert got == want, (where, got, want)
-    assert_same_state(sim, orc, f"after leave, {where}")
-    return got
-
-
-def step(sim, orc, rounds, check=True):
-    sim.step(rounds)
-    orc.step(rounds)
-    if check:
-        assert_same_state(sim, orc, f"round {sim.round}")
-
-
-def pair(n, cap=32, deg=32, kind="random", seed=1, nbr=None, **kw):
-    kw.setdefault("suspicion_rounds", 3)
-    cfg = default_config(n_nodes=n, view_cap=cap, seed=seed, **kw)
-    return make_pair(cfg, generate_topology(kind, n, cap, deg, seed=seed) if nbr is None else nbr)
+leave = partial(B.call, "leave")
 
 
 def leave_list(rng, n, frac=0.03):
@@ -205,9 +188,8 @@ def export_after_leave(n):
 
 def with_push_pull_and_join(n, cap=32, deg=12, seed=10):
     """Leaves, push_pull and joins interleaved, with steps between them."""
-    from join_oracle import join as oracle_join
+    from between_steps_oracle import join as oracle_join, push_pull as oracle_push_pull
     from join_scenarios import restart_pairs
-    from push_pull_oracle import push_pull as oracle_push_pull
     sim, orc = pair(n, cap, deg, seed=seed, loss_ppm=10000)
     rng = np.random.default_rng(seed)
     hosts = rng.choice(n, size=2, replace=False)
@@ -224,86 +206,23 @@ def with_push_pull_and_join(n, cap=32, deg=12, seed=10):
 
 
 def error_paths(n=40):
-    """SWIM_EINVAL on an id >= N, before anything changes; SWIM_ESTATE on a sharded handle that is not connected and
-    before a view is installed."""
-    from swim_b200._lib import SwimError
-    from swim_b200.sim import Simulator
-    sim, orc = pair(n, 32, 10, seed=11)
-    before = sim.state()
-    for ids in ([1, 2, n], [n + 5], [0xFFFFFFFF, 3]):
-        with pytest.raises(SwimError) as e:
-            sim.leave(ids)
-        assert e.value.code == A.EINVAL
-    after = sim.state()
-    assert all(np.array_equal(before[k], after[k]) for k in before)
-    sim.close()
-    shard = Simulator(default_config(n_nodes=n, world=2, rank=0))
-    shard.set_view(generate_topology("random", n, 32, 16, seed=12))
-    bare = Simulator(default_config(n_nodes=n))
-    for s in (shard, bare):
-        with pytest.raises(SwimError) as e:
-            s.leave([1])
-        assert e.value.code == A.ESTATE
-        s.close()
+    """SWIM_EINVAL on an id >= N."""
+    B.error_paths("leave", ([1],), [([1, 2, n],), ([n + 5],), ([0xFFFFFFFF, 3],)], n)
+
+
+sharded_not_connected = partial(B.sharded_not_connected, "leave", ([30],))
 
 
 # ------------------------------------------------------------------ sharded handles
 def sharded_leaves(world, n, mode, devices=None, rounds=24, every=6):
-    """A leave of 3 % of the nodes every `every` rounds on `world` ranks, under events and loss; the shards' sums against
-    the single-shard oracle after every call and every chunk."""
-    import sharded_edit_scenarios as SE
-    sh, orc = SE.setup(world, n, 14, mode, seed=13, devices=devices, rounds=rounds, loss_ppm=10000)
+    """A leave of 3 % of the nodes every `every` rounds on `world` ranks, under events and loss."""
     rng = np.random.default_rng(13)
-    tot = np.zeros(2, dtype=np.int64)
-    for k in range(rounds // every):
-        SE.step(sh, orc, [every])
-        ids = leave_list(rng, n)
-        got, want = sh.total(lambda s: s.leave(ids)), oracle_leave(orc, ids)
-        assert got == want, (k, got, want)
-        sh.check(orc, f"after leave {k}")
-        tot += got
-    SE.step(sh, orc, [1, 3])
-    assert tot[0] > 0 and tot[1] > 0, tot
-    sh.close()
+    B.sharded_every("leave", lambda k: (leave_list(rng, n),), world, n, mode, devices, rounds, every)
 
 
 def sharded_equals_single_shard(n, world, devices, mode="p2p"):
-    """No rounds: at n nodes two leaves of 1 % of the nodes on the shards and on the single-shard handle give the same
-    arrays and totals."""
-    import sharded_edit_scenarios as SE
-    from swim_b200.sim import Simulator
-    kw = SE.config(n, 14, suspicion_rounds=4)
-    nbr = generate_topology("random", n, 32, 16, seed=14)
-    sh = SE.Shards(world, kw, nbr, mode, devices)
-    one = Simulator(default_config(device=devices[0] if devices else -1, **kw))
-    one.set_view(nbr)
-    rng = np.random.default_rng(14)
-    alive = (rng.random(n) > 0.05).astype(np.uint8)
-    one.set_array(A.ARR_ALIVE, alive)
-    for s in sh.sims:
-        s.set_array(A.ARR_ALIVE, alive)
-    for k in range(2):
-        ids = leave_list(rng, n, 0.01)
-        want = one.leave(ids)
-        assert sh.total(lambda s: s.leave(ids)) == want and want[1] > 0, want
-        for a in range(A.ARR_COUNT):
-            assert np.array_equal(sh.array(a), one.get_array(a)), (k, A.ARRAY_NAMES[a])
-    sh.close()
-    one.close()
-
-
-def sharded_not_connected(n=40):
-    from swim_b200._lib import SwimError
-    from swim_b200.sim import Simulator
-    shard = Simulator(default_config(n_nodes=n, world=2, rank=1))
-    shard.set_view(generate_topology("random", n, 32, 16, seed=12))
-    before = shard.state()
-    with pytest.raises(SwimError) as e:
-        shard.leave([30])
-    assert e.value.code == A.ESTATE
-    after = shard.state()
-    assert all(np.array_equal(before[k], after[k]) for k in before)
-    shard.close()
+    """Two leaves of 1 % of the nodes."""
+    B.sharded_equals_single_shard("leave", lambda rng, k: (leave_list(rng, n, 0.01),), n, world, devices, mode)
 
 
 def suspect_turned_dead(n=60, suspicion_max=0):

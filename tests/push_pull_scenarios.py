@@ -1,34 +1,16 @@
 """Scenarios of the push-pull state exchange between steps (swim_sim_push_pull, DESIGN.md 2.6), shared by the emulator
 tests (small sizes) and the H100 tests (2^16 nodes and up). Every call is checked against the CPU oracle: the three
-outputs, every state array, the counters and the digest."""
+outputs, every state array, the counters and the digest (between_steps_scenarios)."""
 import numpy as np
 import pytest
 
-from helpers import assert_same_state, crash_events, default_config, generate_topology, make_pair, random_events
-from push_pull_oracle import push_pull as oracle_push_pull
+from between_steps_scenarios import call, error_paths as _error_paths, pair, step
+from helpers import assert_same_state, crash_events, random_events
 from swim_b200 import _abi as A
-
-NM = A.NO_MEMBER
 
 
 def push_pull(sim, orc, where):
-    got, want = sim.push_pull(), oracle_push_pull(orc)
-    assert got == want, (where, got, want)
-    assert_same_state(sim, orc, f"after push_pull, {where}")
-    return got
-
-
-def step(sim, orc, rounds, check=True):
-    sim.step(rounds)
-    orc.step(rounds)
-    if check:
-        assert_same_state(sim, orc, f"round {sim.round}")
-
-
-def pair(n, cap=32, deg=32, kind="random", seed=1, **kw):
-    kw.setdefault("suspicion_rounds", 3)
-    cfg = default_config(n_nodes=n, view_cap=cap, seed=seed, **kw)
-    return make_pair(cfg, generate_topology(kind, n, cap, deg, seed=seed))
+    return call("push_pull", sim, orc, where=where)
 
 
 def with_events(sim, orc, n, rounds, seed):
@@ -168,15 +150,4 @@ def export_after_push_pull(n):
 
 
 def error_paths(n=40):
-    """SWIM_ESTATE on a sharded handle and before a view is installed; nothing changes."""
-    from swim_b200._lib import SwimError
-    from swim_b200.sim import Simulator
-    nbr = generate_topology("random", n, 32, 16, seed=12)
-    shard = Simulator(default_config(n_nodes=n, world=2, rank=0))
-    shard.set_view(nbr)
-    bare = Simulator(default_config(n_nodes=n))
-    for s in (shard, bare):
-        with pytest.raises(SwimError) as e:
-            s.push_pull()
-        assert e.value.code == A.ESTATE
-        s.close()
+    _error_paths("push_pull", (), n=n)

@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 from helpers import crash_events, default_config, generate_topology, random_events
-from push_pull_oracle import push_pull as oracle_push_pull
+from between_steps_oracle import push_pull as oracle_push_pull
 from spec_fixture import msg
 from swim_b200 import _abi as A
 from view_edit_scenarios import dead_entries, oracle_add, oracle_remove_dead

@@ -3,28 +3,8 @@ library's scalar calls running on the SIMT emulator (tests/emu; the same test on
 import socket
 import time
 
-import pytest
-
-from swim_b200 import _abi as A
-
-
-@pytest.fixture(scope="module", autouse=True)
-def emu_library():
-    import os
-    import sys
-    import swim_b200._lib as L
-    here = os.path.dirname(os.path.abspath(__file__))
-    sys.path.insert(0, os.path.join(here, "emu"))
-    import build_emu
-    so = build_emu.build()
-    saved = (L.SO_PATH, L._lib)
-    L.SO_PATH, L._lib = so, None
-    assert L.lib().swim_abi_version() == A.ABI_VERSION
-    yield
-    L.SO_PATH, L._lib = saved
-
-
 from daemon_scenarios import scenario_live_cluster_detects_a_crash, scenario_probe_escalation_and_relay  # noqa: E402
+from emu_fixtures import emu_library  # noqa: F401  (autouse fixtures)
 
 
 def test_probe_escalation_and_relay():

@@ -7,27 +7,9 @@ import pytest
 
 import leave_scenarios as S
 from swim_b200 import _abi as A
+from emu_fixtures import emu_library, fake_nccl  # noqa: F401  (autouse fixtures)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module", autouse=True)
-def emu_library():
-    import sys
-    import swim_b200._lib as L
-    sys.path.insert(0, os.path.join(ROOT, "tests", "emu"))
-    import build_emu
-    so = build_emu.build()
-    saved = (L.SO_PATH, L._lib)
-    L.SO_PATH, L._lib = so, None
-    assert L.lib().swim_abi_version() == A.ABI_VERSION
-    yield
-    L.SO_PATH, L._lib = saved
-
-
-@pytest.fixture(autouse=True)
-def fake_nccl(monkeypatch):
-    monkeypatch.setenv("SWIM_NCCL_LIB", os.path.join(ROOT, "tests", "emu", "libfake_nccl.so"))
 
 
 @pytest.mark.parametrize("cap", [32, 64, 128, 256])

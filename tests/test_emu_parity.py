@@ -13,22 +13,7 @@ import pytest
 from helpers import assert_same_state, concat_events, crash_events, default_config, generate_topology, make_pair, random_events
 from spec_fixture import member, msg
 from swim_b200 import _abi as A
-
-
-@pytest.fixture(scope="module", autouse=True)
-def emu_library():
-    import os
-    import sys
-    import swim_b200._lib as L
-    here = os.path.dirname(os.path.abspath(__file__))
-    sys.path.insert(0, os.path.join(here, "emu"))
-    import build_emu
-    so = build_emu.build()
-    saved = (L.SO_PATH, L._lib)
-    L.SO_PATH, L._lib = so, None
-    assert L.lib().swim_abi_version() == A.ABI_VERSION
-    yield
-    L.SO_PATH, L._lib = saved
+from emu_fixtures import emu_library  # noqa: F401  (autouse fixtures)
 
 
 def test_c1_every_round():

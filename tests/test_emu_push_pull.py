@@ -4,22 +4,7 @@ import pytest
 
 import push_pull_scenarios as S
 from swim_b200 import _abi as A
-
-
-@pytest.fixture(scope="module", autouse=True)
-def emu_library():
-    import os
-    import sys
-    import swim_b200._lib as L
-    here = os.path.dirname(os.path.abspath(__file__))
-    sys.path.insert(0, os.path.join(here, "emu"))
-    import build_emu
-    so = build_emu.build()
-    saved = (L.SO_PATH, L._lib)
-    L.SO_PATH, L._lib = so, None
-    assert L.lib().swim_abi_version() == A.ABI_VERSION
-    yield
-    L.SO_PATH, L._lib = saved
+from emu_fixtures import emu_library  # noqa: F401  (autouse fixtures)
 
 
 @pytest.mark.parametrize("cap", [32, 64, 128, 256])

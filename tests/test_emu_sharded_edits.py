@@ -1,35 +1,13 @@
 """The bulk membership calls and push-pull on sharded handles, on the SIMT emulator (tests/emu): world 2 and 3, over
 peer memory and through the staged NCCL exchange (tests/emu/fake_nccl.cpp), against the single-shard oracle after every
 call and every chunk of rounds. The H100 versions are in test_gpu_sharded_edits.py."""
-import os
-
 import pytest
 
 import sharded_edit_scenarios as S
 from swim_b200 import _abi as A
+from emu_fixtures import emu_library, fake_nccl  # noqa: F401  (autouse fixtures)
 
 MODES = ["p2p", "nccl"]
-
-
-@pytest.fixture(scope="module", autouse=True)
-def emu_library():
-    import sys
-    import swim_b200._lib as L
-    here = os.path.dirname(os.path.abspath(__file__))
-    sys.path.insert(0, os.path.join(here, "emu"))
-    import build_emu
-    so = build_emu.build()
-    saved = (L.SO_PATH, L._lib)
-    L.SO_PATH, L._lib = so, None
-    assert L.lib().swim_abi_version() == A.ABI_VERSION
-    yield
-    L.SO_PATH, L._lib = saved
-
-
-@pytest.fixture(autouse=True)
-def fake_nccl(monkeypatch):
-    here = os.path.dirname(os.path.abspath(__file__))
-    monkeypatch.setenv("SWIM_NCCL_LIB", os.path.join(here, "emu", "libfake_nccl.so"))
 
 
 @pytest.mark.parametrize("mode", MODES)

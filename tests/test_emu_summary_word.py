@@ -10,21 +10,7 @@ import view_edit_scenarios as S
 from helpers import assert_same_state, concat_events, default_config, generate_topology, make_pair, run_sharded
 from swim_b200 import _abi as A
 from swim_b200.sim import make_events
-
-
-@pytest.fixture(scope="module", autouse=True)
-def emu_library():
-    import os
-    import sys
-    import swim_b200._lib as L
-    here = os.path.dirname(os.path.abspath(__file__))
-    sys.path.insert(0, os.path.join(here, "emu"))
-    import build_emu
-    so = build_emu.build()
-    saved = (L.SO_PATH, L._lib)
-    L.SO_PATH, L._lib = so, None
-    yield
-    L.SO_PATH, L._lib = saved
+from emu_fixtures import emu_library  # noqa: F401  (autouse fixtures)
 
 
 def _inject(sim, orc, ev):

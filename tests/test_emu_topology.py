@@ -4,23 +4,7 @@ of these scenarios are in test_gpu_topology.py."""
 import pytest
 
 import topology_scenarios as T
-from swim_b200 import _abi as A
-
-
-@pytest.fixture(scope="module", autouse=True)
-def emu_library():
-    import os
-    import sys
-    import swim_b200._lib as L
-    here = os.path.dirname(os.path.abspath(__file__))
-    sys.path.insert(0, os.path.join(here, "emu"))
-    import build_emu
-    so = build_emu.build()
-    saved = (L.SO_PATH, L._lib)
-    L.SO_PATH, L._lib = so, None
-    assert L.lib().swim_abi_version() == A.ABI_VERSION
-    yield
-    L.SO_PATH, L._lib = saved
+from emu_fixtures import emu_library  # noqa: F401  (autouse fixtures)
 
 
 @pytest.mark.parametrize("kind,n,cap,deg,seed", [

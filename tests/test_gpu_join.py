@@ -6,7 +6,7 @@ import pytest
 
 import join_scenarios as S
 from helpers import crash_events, default_config, generate_topology, make_pair
-from join_oracle import join as oracle_join
+from between_steps_oracle import join as oracle_join
 from swim_b200 import _abi as A
 
 pytestmark = pytest.mark.gpu

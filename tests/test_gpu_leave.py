@@ -6,7 +6,7 @@ import pytest
 
 import leave_scenarios as S
 from helpers import crash_events, default_config, generate_topology, make_pair
-from leave_oracle import leave as oracle_leave
+from between_steps_oracle import leave as oracle_leave
 from swim_b200 import _abi as A
 
 pytestmark = pytest.mark.gpu

@@ -6,7 +6,7 @@ import pytest
 
 import push_pull_scenarios as S
 from helpers import crash_events, default_config, generate_topology, make_pair
-from push_pull_oracle import push_pull as oracle_push_pull
+from between_steps_oracle import push_pull as oracle_push_pull
 from swim_b200 import _abi as A
 
 pytestmark = pytest.mark.gpu

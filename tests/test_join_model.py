@@ -1,50 +1,27 @@
-"""The C oracle's seed joins (oracle_join in tests/join_oracle.c) against the independent restatement in
-tests/join_model.py (join, over oracle/core_model.py's name-keyed stores) on small graphs: the oracle's state is
-copied into model stores, both run the same pair list, and every view entry, incarnation, piggyback buffer, output and
-counter must agree, under both protocol flags and the Lifeguard timeout."""
+"""The C oracle's seed joins (oracle_join in tests/between_steps_oracle.c) against the independent restatement in
+tests/between_steps_model.py (join, over oracle/core_model.py's name-keyed stores) on small graphs: the oracle's state
+is copied into model stores, both run the same pair list, and every view entry, incarnation, piggyback buffer, output
+and counter must agree, under both protocol flags and the Lifeguard timeout."""
 import numpy as np
 import pytest
 
-from oracle.oracle import Oracle
-from join_model import join as model_join
-from join_oracle import join as oracle_join
+from between_steps_model import assert_same_state, join, name, setup, to_model, up_of, variant
+from between_steps_oracle import join as oracle_join
 from swim_b200 import _abi as A
-from swim_b200.sim import crash_events, default_config, generate_topology
-from test_push_pull_model import lifeguard_deltas, model_arrays, name, oracle_pb, to_model
-
 
 
 def compare(orc, cfg, nodes, seeds, fresh=False):
     """One join on both; returns the oracle's outputs."""
     stores = to_model(orc, cfg)
-    up = {name(i): bool(a) for i, a in enumerate(orc.get_array(A.ARR_ALIVE))}
     c0 = orc.counters()
-    want = model_join(stores, up, [(name(j), name(s)) for j, s in zip(nodes, seeds)], cfg.view_cap, cfg.pb_cap,
-                      cfg.retransmit, fresh, strict=bool(cfg.flags & A.F_STRICT_OVERRIDE), lg_delta=lifeguard_deltas(cfg))
+    want = join(stores, up_of(orc), [(name(j), name(s)) for j, s in zip(nodes, seeds)], cfg.view_cap, cfg.pb_cap,
+                cfg.retransmit, fresh, **variant(cfg))
     got = oracle_join(orc, nodes, seeds, fresh)
     dc = orc.counters() - c0
     assert got == (want["exchanges"], want["inserted"], want["full"])
     assert (dc[A.CTR_RECS_APPLIED], dc[A.CTR_REFUTES], dc[A.CTR_PB_DROPPED]) == (want["applied"], want["refutes"], want["dropped"])
-    nb, st, inc, last, self_inc, pb = model_arrays(stores, cfg)
-    n, cap = cfg.n_nodes, cfg.view_cap
-    assert np.array_equal(orc.get_array(A.ARR_NBR).reshape(n, cap), nb)
-    assert np.array_equal(orc.get_array(A.ARR_VST).reshape(n, cap), st)
-    assert np.array_equal(orc.get_array(A.ARR_VINC).reshape(n, cap), inc)
-    assert np.array_equal(orc.get_array(A.ARR_VLAST).reshape(n, cap), last)
-    assert np.array_equal(orc.get_array(A.ARR_SELF_INC), self_inc)
-    assert oracle_pb(orc, cfg) == pb
+    assert_same_state(orc, stores, cfg)
     return got
-
-
-def setup(n, kind, deg, seed=1, rounds=0, crashes=(), cap=32, **kw):
-    cfg = default_config(n_nodes=n, view_cap=cap, seed=seed, suspicion_rounds=4, **kw)
-    orc = Oracle(cfg)
-    orc.set_view(generate_topology(kind, n, cap, deg, seed=seed))
-    if crashes:
-        orc.inject(crash_events(1, list(crashes)))
-    if rounds:
-        orc.step(rounds)
-    return orc, cfg
 
 
 def test_empty_joiner_rows():

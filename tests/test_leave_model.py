@@ -1,27 +1,22 @@
-"""The C oracle's graceful leaves (oracle_leave in tests/leave_oracle.c) against the independent restatement in
-tests/leave_model.py (leave, over oracle/core_model.py's name-keyed stores) on random views and lists: the oracle's
-state is copied into model stores, both run the same id list, and every view entry, incarnation, piggyback buffer, the
-process arrays, the outputs and the counters must agree, under both protocol flags and the Lifeguard timeout."""
+"""The C oracle's graceful leaves (oracle_leave in tests/between_steps_oracle.c) against the independent restatement in
+tests/between_steps_model.py (leave, over oracle/core_model.py's name-keyed stores) on random views and lists: the
+oracle's state is copied into model stores, both run the same id list, and every view entry, incarnation, piggyback
+buffer, the process arrays, the outputs and the counters must agree, under both protocol flags and the Lifeguard
+timeout."""
 import numpy as np
 import pytest
 
-from oracle.oracle import Oracle
-from leave_model import leave as model_leave
-from leave_oracle import leave as oracle_leave
+from between_steps_model import assert_same_state, leave, name, setup, to_model, up_of, variant
+from between_steps_oracle import leave as oracle_leave
 from swim_b200 import _abi as A
-from swim_b200.sim import crash_events, default_config, generate_topology
-from test_push_pull_model import lifeguard_deltas, model_arrays, name, oracle_pb, to_model
 
 
 def compare(orc, cfg, ids):
     """One leave on both; returns the oracle's outputs."""
     stores = to_model(orc, cfg)
-    n, cap = cfg.n_nodes, cfg.view_cap
-    up = {name(i): bool(a) for i, a in enumerate(orc.get_array(A.ARR_ALIVE))}
     alive, back, crash = (orc.get_array(a).copy() for a in (A.ARR_ALIVE, A.ARR_BACK_AT, A.ARR_LAST_CRASH))
     c0 = orc.counters()
-    want = model_leave(stores, up, [name(int(i)) for i in ids], cfg.pb_cap, cfg.retransmit,
-                       strict=bool(cfg.flags & A.F_STRICT_OVERRIDE), lg_delta=lifeguard_deltas(cfg))
+    want = leave(stores, up_of(orc), [name(int(i)) for i in ids], cfg.pb_cap, cfg.retransmit, **variant(cfg))
     got = oracle_leave(orc, ids)
     dc = orc.counters() - c0
     assert got == (len(want["left"]), want["delivered"])
@@ -31,25 +26,8 @@ def compare(orc, cfg, ids):
     assert np.array_equal(orc.get_array(A.ARR_ALIVE), alive)
     assert np.array_equal(orc.get_array(A.ARR_BACK_AT), back)
     assert np.array_equal(orc.get_array(A.ARR_LAST_CRASH), crash)
-    nb, st, inc, last, self_inc, pb = model_arrays(stores, cfg)
-    assert np.array_equal(orc.get_array(A.ARR_NBR).reshape(n, cap), nb)
-    assert np.array_equal(orc.get_array(A.ARR_VST).reshape(n, cap), st)
-    assert np.array_equal(orc.get_array(A.ARR_VINC).reshape(n, cap), inc)
-    assert np.array_equal(orc.get_array(A.ARR_VLAST).reshape(n, cap), last)
-    assert np.array_equal(orc.get_array(A.ARR_SELF_INC), self_inc)
-    assert oracle_pb(orc, cfg) == pb
+    assert_same_state(orc, stores, cfg)
     return got
-
-
-def setup(n, kind, deg, seed=1, rounds=0, crashes=(), cap=32, **kw):
-    cfg = default_config(n_nodes=n, view_cap=cap, seed=seed, suspicion_rounds=4, **kw)
-    orc = Oracle(cfg)
-    orc.set_view(generate_topology(kind, n, cap, deg, seed=seed))
-    if crashes:
-        orc.inject(crash_events(1, list(crashes)))
-    if rounds:
-        orc.step(rounds)
-    return orc, cfg
 
 
 def test_leavers_that_list_each_other():

@@ -1,123 +1,33 @@
-"""The C oracle's push-pull exchange (tests/push_pull_oracle.c) against the independent restatement in
-tests/push_pull_model.py (over oracle/core_model.py's name-keyed stores, with the reference's own guard order) on small
-graphs: the oracle's state is copied into model stores, both run the exchange, and every view entry, incarnation,
+"""The C oracle's push-pull exchange (tests/between_steps_oracle.c) against the independent restatement in
+tests/between_steps_model.py (over oracle/core_model.py's name-keyed stores, with the reference's own guard order) on
+small graphs: the oracle's state is copied into model stores, both run the exchange, and every view entry, incarnation,
 piggyback buffer, output and counter must agree, under both protocol flags and the Lifeguard timeout."""
 import numpy as np
 import pytest
 
-from oracle import core_model as M
+from between_steps_model import assert_same_state, push_pull, setup, to_model, up_of, variant
+from between_steps_oracle import push_pull as oracle_push_pull
 from oracle.oracle import Oracle, philox
-from push_pull_model import push_pull as model_push_pull
-from push_pull_oracle import push_pull as oracle_push_pull
 from swim_b200 import _abi as A
-from swim_b200.sim import crash_events, default_config, generate_topology
+from swim_b200.sim import default_config
 
 NM = A.NO_MEMBER
-KIND = {A.MSG_ALIVE: "Alive", A.MSG_SUSPECT: "Suspect", A.MSG_DEAD: "Dead"}
-
-
-def name(i):
-    return f"{i:05d}"  # key order == id order
-
-
-def lifeguard_deltas(cfg):
-    """What the c-th confirmation takes off a countdown: timeout(c) = max - (max - min) log(c + 1) / log 4, c = 0..3, in
-    256ths rounded (the oracle's table)."""
-    if not cfg.suspicion_max:
-        return None
-    frac = (0, 128, 203, 256)
-    T = [cfg.suspicion_max - ((cfg.suspicion_max - cfg.suspicion_rounds) * f + 128) // 256 for f in frac]
-    return [0] + [T[c - 1] - T[c] for c in range(1, 4)]
-
-
-def to_model(orc, cfg):
-    n, cap = cfg.n_nodes, cfg.view_cap
-    lg = cfg.suspicion_max != 0
-    nb, st, inc, last = (orc.get_array(a).reshape(n, cap) for a in (A.ARR_NBR, A.ARR_VST, A.ARR_VINC, A.ARR_VLAST))
-    pb, cnt = orc.get_array(A.ARR_PB).reshape(n, cfg.pb_cap), orc.get_array(A.ARR_PB_CNT)
-    stores = {}
-    for i in range(n):
-        s = M.Store(M.Member(name(i)), cfg.suspicion_max or cfg.suspicion_rounds)
-        s.conf = {}
-        s.incarnation = int(orc.get_array(A.ARR_SELF_INC)[i])
-        s.now = orc.round
-        for x in range(cap):
-            if st[i, x] & 3 == A.VACANT:
-                continue
-            m = name(int(nb[i, x]))
-            s.members[m] = M.Member(m, "", 0, 0, int(st[i, x] & 3), int(inc[i, x]), int(last[i, x]))
-            if st[i, x] & 3 == A.SUSPECT:
-                s.timers[m] = (int(st[i, x]) >> 2) & (15 if lg else 63)
-                if lg and st[i, x] >> 6:
-                    s.conf[m] = int(st[i, x]) >> 6
-        s.queue = [(M.Msg(KIND[int(r["kind"])], node=name(int(r["member"])), incarnation=int(r["incarnation"]),
-                          dead_from=name(int(r["from"])) if r["kind"] == A.MSG_DEAD else ""), int(r["ttl"]))
-                   for r in pb[i, : cnt[i]]]
-        stores[name(i)] = s
-    return stores
-
-
-def model_arrays(stores, cfg):
-    n, cap = cfg.n_nodes, cfg.view_cap
-    nb = np.full((n, cap), NM, np.uint32)
-    st = np.full((n, cap), A.VACANT, np.uint8)
-    inc = np.zeros((n, cap), np.uint32)
-    last = np.zeros((n, cap), np.uint32)
-    pb = []
-    for i in range(n):
-        s = stores[name(i)]
-        for x, m in enumerate(M.members(s)):
-            nb[i, x], inc[i, x], last[i, x] = int(m.name), m.incarnation, m.last_change
-            if m.alive == A.SUSPECT:
-                st[i, x] = m.alive | (s.timers.get(m.name, 0) << 2) | (s.conf.get(m.name, 0) << 6)
-            else:
-                st[i, x] = m.alive
-        pb.append([(int(m.node), {"Alive": A.MSG_ALIVE, "Suspect": A.MSG_SUSPECT, "Dead": A.MSG_DEAD}[m.kind],
-                    m.incarnation, int(m.dead_from) if m.kind == "Dead" else 0, t) for m, t in s.queue])
-    self_inc = np.array([stores[name(i)].incarnation for i in range(n)], np.uint32)
-    return nb, st, inc, last, self_inc, pb
-
-
-def oracle_pb(orc, cfg):
-    pb, cnt = orc.get_array(A.ARR_PB).reshape(cfg.n_nodes, cfg.pb_cap), orc.get_array(A.ARR_PB_CNT)
-    return [[(int(r["member"]), int(r["kind"]), int(r["incarnation"]), int(r["from"]), int(r["ttl"])) for r in pb[i, : cnt[i]]]
-            for i in range(cfg.n_nodes)]
 
 
 def compare(orc, cfg):
     """One exchange on both; returns the oracle's outputs."""
     stores = to_model(orc, cfg)
-    up = {name(i): bool(a) for i, a in enumerate(orc.get_array(A.ARR_ALIVE))}
     key = (cfg.seed & 0xFFFFFFFF, cfg.seed >> 32)
     r = orc.round
     draw = lambda k: philox([r, int(k), 10, 0], key)[0]
     c0 = orc.counters()
-    want = model_push_pull(stores, up, draw, cfg.view_cap, cfg.pb_cap, cfg.retransmit,
-                           strict=bool(cfg.flags & A.F_STRICT_OVERRIDE), lg_delta=lifeguard_deltas(cfg))
+    want = push_pull(stores, up_of(orc), draw, cfg.view_cap, cfg.pb_cap, cfg.retransmit, **variant(cfg))
     got = oracle_push_pull(orc)
     dc = orc.counters() - c0
     assert got == (want["exchanges"], want["inserted"], want["full"])
     assert (dc[A.CTR_RECS_APPLIED], dc[A.CTR_REFUTES], dc[A.CTR_PB_DROPPED]) == (want["applied"], want["refutes"], want["dropped"])
-    nb, st, inc, last, self_inc, pb = model_arrays(stores, cfg)
-    n, cap = cfg.n_nodes, cfg.view_cap
-    assert np.array_equal(orc.get_array(A.ARR_NBR).reshape(n, cap), nb)
-    assert np.array_equal(orc.get_array(A.ARR_VST).reshape(n, cap), st)
-    assert np.array_equal(orc.get_array(A.ARR_VINC).reshape(n, cap), inc)
-    assert np.array_equal(orc.get_array(A.ARR_VLAST).reshape(n, cap), last)
-    assert np.array_equal(orc.get_array(A.ARR_SELF_INC), self_inc)
-    assert oracle_pb(orc, cfg) == pb
+    assert_same_state(orc, stores, cfg)
     return got
-
-
-def setup(n, kind, deg, seed=1, rounds=0, crashes=(), cap=32, **kw):
-    cfg = default_config(n_nodes=n, view_cap=cap, seed=seed, suspicion_rounds=4, **kw)
-    orc = Oracle(cfg)
-    orc.set_view(generate_topology(kind, n, cap, deg, seed=seed))
-    if crashes:
-        orc.inject(crash_events(1, list(crashes)))
-    if rounds:
-        orc.step(rounds)
-    return orc, cfg
 
 
 @pytest.mark.parametrize("kind,deg,n", [("complete", 32, 12), ("ring", 2, 16), ("ring", 6, 16), ("random", 5, 16)])

@@ -7,7 +7,7 @@ import os
 import numpy as np
 import pytest
 
-from leave_oracle import leave as oracle_leave
+from between_steps_oracle import leave as oracle_leave
 from oracle.oracle import Oracle
 from swim_b200 import _abi as A
 from swim_b200.sim import default_config, generate_topology
