@@ -63,10 +63,11 @@ def error_paths(name, args, invalid=(), n=40):
 
 
 # ------------------------------------------------------------------ sharded handles
-def sharded_every(name, args, world, n, mode, devices=None, rounds=24, every=6):
+def sharded_every(name, args, world, n, mode, devices=None, rounds=24, every=6, **kw):
     """The call with args(k) every `every` rounds on `world` ranks, under events and loss; the shards' sums against the
-    single-shard oracle after every call and every chunk. The first two outputs, summed, are positive."""
-    sh, orc = SE.setup(world, n, 14, mode, seed=13, devices=devices, rounds=rounds, loss_ppm=10000)
+    single-shard oracle after every call and every chunk. The first two outputs, summed, are positive. `kw` overrides
+    config fields (the view is generated at its view_cap)."""
+    sh, orc = SE.setup(world, n, 14, mode, seed=13, devices=devices, rounds=rounds, **{"loss_ppm": 10000, **kw})
     tot = 0
     for k in range(rounds // every):
         SE.step(sh, orc, [every])
@@ -80,12 +81,12 @@ def sharded_every(name, args, world, n, mode, devices=None, rounds=24, every=6):
     sh.close()
 
 
-def sharded_equals_single_shard(name, args, n, world, devices, mode="p2p"):
+def sharded_equals_single_shard(name, args, n, world, devices, mode="p2p", **kw):
     """No rounds: at n nodes, with 5 % of them down, two calls with args(rng, k) on the shards and on the single-shard
-    handle give the same arrays and totals, and the second output is positive."""
+    handle give the same arrays and totals, and the second output is positive. `kw` overrides config fields."""
     from swim_b200.sim import Simulator
-    kw = SE.config(n, 14, suspicion_rounds=4)
-    nbr = generate_topology("random", n, 32, 16, seed=14)
+    kw = SE.config(n, 14, **{"suspicion_rounds": 4, **kw})
+    nbr = generate_topology("random", n, kw.get("view_cap", 32), 16, seed=14)
     sh = SE.Shards(world, kw, nbr, mode, devices)
     one = Simulator(default_config(device=devices[0] if devices else -1, **kw))
     one.set_view(nbr)

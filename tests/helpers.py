@@ -54,20 +54,22 @@ def random_events(rng, n_nodes, rounds, n_crash, n_rejoin=0, n_inject=0):
     return concat_events(evs)
 
 
-def run_sharded(world, n, chunks, loss, deg, flags=0, mode="p2p", devices=None, churn=None):
+def run_sharded(world, n, chunks, loss, deg, flags=0, mode="p2p", devices=None, churn=None, **overrides):
     """`world` handles in ONE process — on the emulator `world` emulated GPUs, on hardware all ranks on one device (or
     devices[r]): ranks of one process connect through raw device pointers (swim_sim_ipc_export / _connect), so the peers'
     arrays are addressed exactly as over NVLink. Each rank steps on its own host thread (its kernels wait for the others
-    on the device); the sum of the shards must be the single-shard oracle's state."""
+    on the device); the sum of the shards must be the single-shard oracle's state. `overrides` replace config fields
+    (view_cap, k_indirect, fanout, pb_cap, ...); the view is generated at that view_cap."""
     from oracle.oracle import Oracle
     from swim_b200.sim import Simulator
     rng = np.random.default_rng(world * 100 + n)
-    nbr = generate_topology("random", n, 32, deg, seed=6)
-    total = sum(chunks)
-    events = random_events(rng, n, total, n_crash=max(2, n // 12), n_rejoin=max(1, n // 40), n_inject=n // 10)
     kw = dict(n_nodes=n, k_indirect=3, fanout=4, pb_cap=6, suspicion_rounds=4, retransmit=5, loss_ppm=loss, seed=4242, flags=flags)
     if churn:
         kw.update(churn_ppm=churn[0], rejoin_min=churn[1], rejoin_max=churn[2])
+    kw.update(overrides)
+    nbr = generate_topology("random", n, kw.get("view_cap", 32), deg, seed=6)
+    total = sum(chunks)
+    events = random_events(rng, n, total, n_crash=max(2, n // 12), n_rejoin=max(1, n // 40), n_inject=n // 10)
     sims = [Simulator(default_config(rank=r, world=world, device=(devices[r] if devices else -1), **kw)) for r in range(world)]
     for s in sims:
         s.set_view(nbr)

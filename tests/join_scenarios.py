@@ -207,16 +207,17 @@ sharded_not_connected = partial(B.sharded_not_connected, "join", ([30], [1], Tru
 
 
 # ------------------------------------------------------------------ sharded handles
-def sharded_joins(world, n, mode, devices=None, rounds=24, every=6):
-    """Joins through 3 seeds every `every` rounds on `world` ranks, alternately fresh and not, under events and loss."""
+def sharded_joins(world, n, mode, devices=None, rounds=24, every=6, **kw):
+    """Joins through 3 seeds every `every` rounds on `world` ranks, alternately fresh and not, under events and loss.
+    `kw` overrides config fields."""
     rng = np.random.default_rng(13)
     hosts = rng.choice(n, size=3, replace=False)
     B.sharded_every("join", lambda k: (*restart_pairs(rng, n, hosts), k % 2 == 1), world, n, mode, devices, rounds,
-                    every)
+                    every, **kw)
 
 
-def sharded_equals_single_shard(n, world, devices, mode="p2p"):
+def sharded_equals_single_shard(n, world, devices, mode="p2p", **kw):
     """A fresh join of 1 % of the nodes through 3 seeds, then a plain one."""
     B.sharded_equals_single_shard(
         "join", lambda rng, k: (*restart_pairs(rng, n, rng.choice(n, size=3, replace=False), 0.01), k == 0), n, world,
-        devices, mode)
+        devices, mode, **kw)

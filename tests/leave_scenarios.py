@@ -214,15 +214,16 @@ sharded_not_connected = partial(B.sharded_not_connected, "leave", ([30],))
 
 
 # ------------------------------------------------------------------ sharded handles
-def sharded_leaves(world, n, mode, devices=None, rounds=24, every=6):
-    """A leave of 3 % of the nodes every `every` rounds on `world` ranks, under events and loss."""
+def sharded_leaves(world, n, mode, devices=None, rounds=24, every=6, **kw):
+    """A leave of 3 % of the nodes every `every` rounds on `world` ranks, under events and loss. `kw` overrides config
+    fields."""
     rng = np.random.default_rng(13)
-    B.sharded_every("leave", lambda k: (leave_list(rng, n),), world, n, mode, devices, rounds, every)
+    B.sharded_every("leave", lambda k: (leave_list(rng, n),), world, n, mode, devices, rounds, every, **kw)
 
 
-def sharded_equals_single_shard(n, world, devices, mode="p2p"):
+def sharded_equals_single_shard(n, world, devices, mode="p2p", **kw):
     """Two leaves of 1 % of the nodes."""
-    B.sharded_equals_single_shard("leave", lambda rng, k: (leave_list(rng, n, 0.01),), n, world, devices, mode)
+    B.sharded_equals_single_shard("leave", lambda rng, k: (leave_list(rng, n, 0.01),), n, world, devices, mode, **kw)
 
 
 def suspect_turned_dead(n=60, suspicion_max=0):

@@ -111,10 +111,11 @@ def config(n, seed, **kw):
 
 
 def setup(world, n, deg, mode, seed, devices=None, events=True, rounds=20, **kw):
-    """Shards and the single-shard oracle on one random view, with the same event trace."""
+    """Shards and the single-shard oracle on one random view, with the same event trace. `kw` overrides config fields;
+    the view is generated at its view_cap (32 by default)."""
     from oracle.oracle import Oracle
     kw = config(n, seed, **kw)
-    nbr = generate_topology("random", n, 32, deg, seed=seed)
+    nbr = generate_topology("random", n, kw.get("view_cap", 32), deg, seed=seed)
     sh = Shards(world, kw, nbr, mode, devices)
     orc = Oracle(default_config(**kw))
     orc.set_view(nbr)
@@ -140,9 +141,9 @@ def push_pull(sh, orc, where):
     return got
 
 
-def remove_dead_then_rounds(world, n, mode, devices=None, chunks=(1, 1, 4, 10)):
+def remove_dead_then_rounds(world, n, mode, devices=None, chunks=(1, 1, 4, 10), **kw):
     """removeDeadNodes on every store of every rank, then rounds (the first one rebuilds the mail graph together)."""
-    sh, orc = setup(world, n, 24, mode, seed=3, devices=devices, loss_ppm=20000)
+    sh, orc = setup(world, n, 24, mode, seed=3, devices=devices, **{"loss_ppm": 20000, **kw})
     step(sh, orc, [6, 14])
     want = dead_entries(orc)
     assert want > 0
@@ -182,10 +183,10 @@ def remove_dead_min_age(world, n, mode, min_age, devices=None, chunks=(1, 3, 8))
     one.close()
 
 
-def add_members_then_rounds(world, n, mode, devices=None, chunks=(1, 2, 8)):
+def add_members_then_rounds(world, n, mode, devices=None, chunks=(1, 2, 8), deg=26, **kw):
     """The same global add list on every rank; each applies the adds of its own observers. Adds to full rows, adds whose
     observer lies on another rank than the member, known members and duplicates within the call."""
-    sh, orc = setup(world, n, 26, mode, seed=5, devices=devices, events=False, loss_ppm=10000)
+    sh, orc = setup(world, n, deg, mode, seed=5, devices=devices, events=False, **{"loss_ppm": 10000, **kw})
     ev = crash_events(2, np.random.default_rng(5).choice(n, size=max(1, n // 30), replace=False))
     sh.inject(ev)
     orc.inject(ev)
@@ -197,7 +198,7 @@ def add_members_then_rounds(world, n, mode, devices=None, chunks=(1, 2, 8)):
     obs[k // 4: k // 2] = n - 1  # the last shard's last row (the smallest shard, when the split is uneven)
     mem = rng.integers(0, n, size=k)
     mem[obs == mem] = (mem[obs == mem] + 1) % n
-    known = orc.get_array(A.ARR_NBR).reshape(n, 32)[obs[3 * k // 4:], 0]  # slot 0 of a row: a member it lists
+    known = orc.get_array(A.ARR_NBR).reshape(n, -1)[obs[3 * k // 4:], 0]  # slot 0 of a row: a member it lists
     mem[3 * k // 4:] = np.where(known != NM, known, mem[3 * k // 4:])
     mem[-3:], obs[-3:] = mem[-4], obs[-4]  # duplicates within the call
     inc = rng.integers(0, 5, size=k)
@@ -225,9 +226,10 @@ def push_pull_inserts_then_rounds(world, n, mode, devices=None, rounds=50, chunk
     sh.close()
 
 
-def push_pull_every(world, n, mode, rounds=24, every=6, devices=None, flags=0, churn=None, loss=20000, suspicion_max=0):
+def push_pull_every(world, n, mode, rounds=24, every=6, devices=None, flags=0, churn=None, loss=20000, suspicion_max=0,
+                    **overrides):
     """push_pull every `every` rounds under events, device churn and loss, in the protocol variants."""
-    kw = dict(loss_ppm=loss, flags=flags, suspicion_max=suspicion_max)
+    kw = dict(loss_ppm=loss, flags=flags, suspicion_max=suspicion_max, **overrides)
     if churn:
         kw.update(churn_ppm=churn[0], rejoin_min=churn[1], rejoin_max=churn[2])
     sh, orc = setup(world, n, 20, mode, seed=7, devices=devices, rounds=rounds, **kw)

@@ -7,6 +7,7 @@ import pytest
 import leave_scenarios as S
 from helpers import crash_events, default_config, generate_topology, make_pair
 from between_steps_oracle import leave as oracle_leave
+from nccl_fixtures import fake_nccl_gpu, fake_nccl_gpu_lib, staged_too  # noqa: F401  (fixtures)
 from swim_b200 import _abi as A
 
 pytestmark = pytest.mark.gpu
@@ -88,9 +89,12 @@ def test_c3_leaves_every_25_rounds():
 
 
 @pytest.mark.usefixtures("fused_exchange")
-@pytest.mark.parametrize("world", [2, 3, 4])
-def test_sharded(world):
-    S.sharded_leaves(world, 1100, "p2p", devices=[0] * world, rounds=36, every=12)
+@pytest.mark.parametrize("world,mode", staged_too([2, 3, 4], ["2", "3", "4"]))
+def test_sharded(world, mode, request):
+    """Over peer memory, and through the staged exchange with the in-process NCCL stand-in ("nccl")."""
+    if mode == "nccl":
+        request.getfixturevalue("fake_nccl_gpu")
+    S.sharded_leaves(world, 1100, mode, devices=[0] * world, rounds=36, every=12)
 
 
 def test_sharded_equals_single_shard():
